@@ -93,7 +93,7 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "fallback (H100 SXM data sheet)"
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -303,15 +303,9 @@ def run_ours(args):
     ach = (alg_bytes * (n_timed / max(1, n_launch))) / max(1e-9, ns * 1e-9) / 1e9 if n_timed else 0.0
     roof = {"kernel": "TSDF stencil (stencil_multi_kernel: a frame's re-integration batch in one pass; stencil_fast_kernel: single integrate)" if scene.arithmetic == "fast" else "integrate_kernel / reintegrate_kernel (bit-exact TSDF stencil)", "bound": "hbm", "achieved": round(ach, 1), "peak": peaks["hbm_gbs"],
             "peak_kind": f"{peak_kind} (MEASURED_PEAKS.json hbm_gbs, burst copy)", "unit": "GB/s", "frac": round(ach / peaks["hbm_gbs"], 4),
-            "traffic": None, "launches": n_launch, "avg_launch_us": round(ns / max(1, n_timed) / 1e3, 2),
+            "launches": n_launch, "avg_launch_us": round(ns / max(1, n_timed) / 1e3, 2),
             "algorithmic_bytes_per_launch": round(alg_bytes / max(1, n_launch)), "U_per_launch": round(U / max(1, n_launch)), "E_per_launch": round(E / max(1, n_launch)),
             "frames_per_launch": round(n_img / max(1, n_launch), 2), "all_stencil_launches": all_launches}
-    # DRAM traffic of the dominant kernel from the committed `ncu --set full` capture of this command (profiles/), per launch
-    tpath = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r1_stencil_traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        roof["traffic"] = tj.get("dram_bytes_per_launch")
-        roof["traffic_note"] = tj.get("note")
     bytes_in = (W * H * 4 * 2)
     bytes_out = 4 + (6 * 4 * len(glo["init_rot"])) / WORKLOAD["chunk"]
     out = {
@@ -394,6 +388,8 @@ def run_loop(args):
             note(st)
     torch.cuda.synchronize()
 
+    last = {}
+
     def timed(f0, n, e2e, profile):
         if world > 1:
             dist.barrier()
@@ -413,6 +409,7 @@ def run_loop(args):
                 st = loop.step(depth[f0 + k], color[f0 + k], *((depth[f0 + k + 1], color[f0 + k + 1]) if la else (None, None)))
             if not profile:
                 note(st)
+            last["status"] = st
             if steptimes is not None:
                 steptimes.append((int(st.frame), round((time.perf_counter() - t_step0) * 1e3, 3), int(st.localSolved), int(st.globalSolved), int(st.globalRemoved), int(st.numKeyframes)))
         if steptimes is not None and rank == 0:             # diagnostic: host wall time of every step call of this pass
@@ -434,6 +431,8 @@ def run_loop(args):
     ms, launches = timed(pre + Wm, K, False, False)
     if args.cuda_profiler:
         torch.cuda.profiler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_loop_outputs(args.dump_outputs, last["status"], loop.trajectory(pre + Wm + K))
     clk_mark1 = len(clk_lines)
     c_before = loop.counters()
     prev_lanes = L.bfTsdfSetLanes(0)                       # the stencil is timed alone on its stream: the burst HBM peak is its roof
@@ -471,16 +470,13 @@ def run_loop(args):
     ach = (alg_bytes * (n_timed / max(1, n_launch))) / max(1e-9, ns * 1e-9) / 1e9 if n_timed else 0.0
     roof = {"kernel": "stencil_multi_kernel (TSDF stencil: a frame's re-integration batch, every voxel of the union list read and written once)" if use_batch else "stencil_fast_kernel",
             "bound": "hbm", "achieved": round(ach, 1), "peak": peaks["hbm_gbs"], "peak_kind": f"{peak_kind} (MEASURED_PEAKS.json hbm_gbs, burst copy)", "unit": "GB/s",
-            "frac": round(ach / peaks["hbm_gbs"], 4), "traffic": None, "launches": n_launch, "avg_launch_us": round(ns / max(1, n_timed) / 1e3, 2),
+            "frac": round(ach / peaks["hbm_gbs"], 4), "launches": n_launch, "avg_launch_us": round(ns / max(1, n_timed) / 1e3, 2),
             "algorithmic_bytes_per_launch": round(alg_bytes / max(1, n_launch)), "U_per_launch": round(U / max(1, n_launch)), "E_per_launch": round(E / max(1, n_launch)),
             "frames_per_launch": round(n_img / max(1, n_launch), 2),
             "avg_launch_us_device_timer": round(int(prof[14]) / max(1, n_timed) / 1e3, 2) if use_batch and int(prof[14]) else None,
             "all_stencil_launches": {"launches": int(prof[0]), "avg_launch_us": round(int(prof[2]) / max(1, int(prof[1])) / 1e3, 2)},
             "mvoxels_per_s": round(512.0 * E / max(1e-9, ns * 1e-9) / 1e6, 1),
             "block_pose_entries_culled_per_launch": round(int(prof[15]) / max(1, n_launch)) if use_batch else None}
-    tpath = os.path.join(ROOT, "profiles", "r2_stencil_traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath)); roof["traffic"] = tj.get("dram_bytes_per_launch"); roof["traffic_note"] = tj.get("note")
     steps_meas = max(1, stats["n"])
     out = {
         "metric": METRIC, "value": round(K / (ms / 1e3), 2), "unit": "frames/s", "n_gpus": world, "steps": K, "warmup": Wm,
@@ -516,6 +512,16 @@ def run_loop(args):
     print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+def dump_loop_outputs(out_dir, status, trajectory):
+    """what a caller of the frame loop holds after the timed pass's last step: that step's status block (the frame's pose, and its scalar
+    fields in BFFrameLoopStatus order as float64) and the trajectory of every frame streamed so far"""
+    os.makedirs(out_dir, exist_ok=True)
+    d = status.as_dict()
+    np.save(os.path.join(out_dir, "last_pose.npy"), d.pop("transform").astype(np.float32))
+    np.save(os.path.join(out_dir, "last_status.npy"), np.array([float(d[n]) for n, _ in status._fields_ if n != "transform"], np.float64))
+    np.save(os.path.join(out_dir, "trajectory.npy"), np.ascontiguousarray(trajectory, np.float32))
+
 
 # ------------------------------------------------------------------------------------------------------------------------
 def run_sweep(args):
@@ -678,7 +684,7 @@ def mesh_leg(L, loop, P, dev, active_blocks):
 
 def reference_cuda_leg(dev, n_frames=12):
     """The reference's OWN CUDA for the TSDF + bundle-adjustment share of a step -- its kernels and host loops (oracle/_ref: the reference sources
-    compiled for sm_100a with --use_fast_math, as it ships), driven exactly like this library on the same inputs, same box, same run: per frame
+    compiled for sm_90a with --use_fast_math, as it ships), driven exactly like this library on the same inputs, same box, same run: per frame
     1 integrate + 10 x (de-integrate + integrate) + garbage collection; per 10 frames one local BA (11 frames, sparse + dense, 2 x 100) and one global BA
     (500 keyframes, sparse, 3 x 150).  Wall clock with a device synchronise on both sides (the reference's host loops synchronise internally).
     A reported baseline like cpu_baseline: bounded sample, rank 0, N = 1."""
@@ -780,7 +786,7 @@ def reference_cuda_leg(dev, n_frames=12):
             o[k] = round(o[k], 3)
     return {"value": out["reference_cuda"]["frames_per_s"], "unit": "frames/s", "this_repo_same_sample": out["this_repo"]["frames_per_s"],
             "speedup": round(out["this_repo"]["frames_per_s"] / out["reference_cuda"]["frames_per_s"], 2), "parts": out, "pcg": pcg_info,
-            "kind": "the reference's CUDA kernels and host loops (oracle/_ref: its sources built for sm_100a with --use_fast_math) on this box, TSDF + bundle-adjustment share of a step (the stages the reference's stub surface covers), serial on one stream, wall clock",
+            "kind": "the reference's CUDA kernels and host loops (oracle/_ref: its sources built for sm_90a with --use_fast_math) on this box, TSDF + bundle-adjustment share of a step (the stages the reference's stub surface covers), serial on one stream, wall clock",
             "sample": f"{n_frames} frames of 1 integrate + 10 re-integrations + GC at 1 cm voxels; 3 repetitions of the local (11 frames, sparse + dense) and global (500 keyframes) solves"}
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -862,13 +868,13 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    K, Wm = max(1, min(args.steps, 6)), min(args.warmup, 1)
+    K, Wm = max(1, args.steps), min(args.warmup, 1)
     t0 = time.perf_counter()
     base = cpu_arm(K, Wm, n_reint=WORKLOAD["reintegrations_per_frame"])
     wall = time.perf_counter() - t0
     out = {"impl": "reference", "metric": METRIC, "value": base["value"], "unit": "frames/s", "n_gpus": int(os.environ.get("WORLD_SIZE", "1")),
            "steps": K, "warmup": Wm, "ms_per_step": round(1e3 / base["value"], 2), "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-           "dtype": "f32", "data": "synthetic", "config": dict(LOOP_WORKLOAD, note="CPU arm: oracle port of the reference algorithm on the host cores (the reference ships no CPU path of its own; its CUDA path, rebuilt for sm_100a, is timed in the default arm's `reference_cuda` entry).  It times the stages of the default arm's step by bounded samples -- per frame 1 integrate + 10 re-integrations + GC, ingest, SIFT detection, dense cache, descriptor matching against the chunk; per 10 frames one local and one global solve and the keyframe matching -- and adds them up; the match filters (sub-millisecond per frame on one core) and the host sequencing are left out"),
+           "dtype": "f32", "data": "synthetic", "config": dict(LOOP_WORKLOAD, note="CPU arm: oracle port of the reference algorithm on the host cores (the reference ships no CPU path of its own; its CUDA path, rebuilt for sm_90a, is timed in the default arm's `reference_cuda` entry).  It times the stages of the default arm's step by bounded samples -- per frame 1 integrate + 10 re-integrations + GC, ingest, SIFT detection, dense cache, descriptor matching against the chunk; per 10 frames one local and one global solve and the keyframe matching -- and adds them up; the match filters (sub-millisecond per frame on one core) and the host sequencing are left out"),
            "cpu_baseline": base, "e2e": {"value": base["value"], "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}, "wall_s": round(wall, 1)}
     print(json.dumps(out))
 
@@ -886,7 +892,10 @@ def main():
     ap.add_argument("--preroll", type=int, default=250, help="frames streamed through the loop before warm-up (state of a long stream)")
     ap.add_argument("--trace", default=None, help="diagnostic: write the per-frame status of every step (pre-roll included) to this file")
     ap.add_argument("--stride", type=int, default=2, help="Lissajous path frames per step")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="loop workload: write what the timed pass's last step returned (pose, status, trajectory) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "loop"):
+        ap.error("--dump-outputs writes the outputs of the frame loop: it needs the default --impl ours --workload loop")
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-// cache.cu -- dense-cache frame builder for sm_100a.  Implements include/bf_cache.h (row a20 of SURVEY.md section 8).
+// cache.cu -- dense-cache frame builder for sm_90a.  Implements include/bf_cache.h (row a20 of SURVEY.md section 8).
 //
 // Behavioural source (what, not how): FL/CUDACache.cpp:45-86 and the eight FL/CUDAImageUtil.cu kernels it calls (listed in the
 // header).  The reference filters, back-projects and takes normals of the WHOLE 640x480 image (3 full-resolution float / float4

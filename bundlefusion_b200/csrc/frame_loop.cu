@@ -892,7 +892,7 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
         e = cudaMallocHost(&L.h_complete, sizeof(float) * 16 * (size_t)P.maxNumFrames);
         if (e != cudaSuccess) { rc = (int)e; break; }
         // Library-private workspaces at their final size NOW: growing one later means cudaFree + cudaMalloc in the middle of a frame, and with the loop's other
-        // streams busy that was measured as a single 0.5 s stall (profiles/r2_lookahead_stall_steptimes.txt).  Matcher: one job per keyframe at most;
+        // streams busy that shows up as a single long stall.  Matcher: one job per keyframe at most;
         // solvers: the chunk's and the keyframe set's residual capacities (the keyframe solver's capped at 1 M entries up front, it doubles beyond)
         if ((rc = bfSiftReserveWorkspace(std::max(P.maxNumImages, P.submapSize + 1), P.maxNumKeysPerImage))) break;
         if ((rc = bfSolverReserveWorkspace(&L.local.solver.st, L.local.solver.maxImages, L.local.solver.maxResiduals, P.useLocalDense ? 1 : 0))) break;

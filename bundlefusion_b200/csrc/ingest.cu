@@ -1,4 +1,4 @@
-// ingest.cu -- per-frame sensor-image preparation for sm_100a.  Implements include/bf_ingest.h (row a21 of SURVEY.md section 8).
+// ingest.cu -- per-frame sensor-image preparation for sm_90a.  Implements include/bf_ingest.h (row a21 of SURVEY.md section 8).
 //
 // Behavioural source (what, not how): FL/CUDAImageManager.cpp:44-61, 88-137 and FL/CUDAImageUtil.cu erodeDepthMapDevice (:701-741),
 // gaussFilterDepthMapDevice (:759-794), resampleFloat_Kernel (:93-110), resampleUCHAR4_Kernel (:160-177).

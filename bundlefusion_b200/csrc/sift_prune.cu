@@ -1,10 +1,9 @@
-// sift_prune.cu -- correspondence / frame invalidation after a solve, for sm_100a (the device half of SBA::removeMaxResidualCUDA,
+// sift_prune.cu -- correspondence / frame invalidation after a solve, for sm_90a (the device half of SBA::removeMaxResidualCUDA,
 // FL/SBA.cpp:165-203; rows a16 / a19).  Implements bfSiftInvalidateImageToImage and bfSiftCheckForInvalidFrames of include/bf_sift.h.
 //
 // Behavioural source (what, not how): InvalidateImageToImageCU_Kernel / CheckForInvalidFramesSimpleCU_Kernel /
 // CheckForInvalidFramesCU_Kernel, FL/SiftGPU/SIFTImageManager.cu:692-790.  Integer work, bit-exact.
-// STATUS: compiled for sm_100a and verified under the CPU emulation of tests/cuda_emu (tests/test_sift_prune_emulated.py); not yet
-// run on hardware -- tests/test_zz_sift_prune_gpu.py is committed for its first hardware run.
+// Verified under the CPU emulation of tests/cuda_emu (tests/test_sift_prune_emulated.py) and on the GPU (tests/test_zz_sift_prune_gpu.py).
 #include "../../include/bf_sift.h"
 #include "bf_common.cuh"
 

@@ -1,4 +1,4 @@
-// sift_verify.cu -- the two match filters that follow the Kabsch filter, for sm_100a (row a19, second and third filter):
+// sift_verify.cu -- the two match filters that follow the Kabsch filter, for sm_90a (row a19, second and third filter):
 // bfSiftFilterMatchesBySurfaceArea and bfSiftFilterMatchesByDenseVerify of include/bf_sift.h.
 //
 // Behavioural source (what, not how): FL/SiftGPU/SIFTImageManager.cu:318-407 (FilterMatchesBySurfaceAreaCU) with

@@ -1,10 +1,10 @@
-// solver.cu -- sparse bundle adjustment (Gauss-Newton + Jacobi-PCG in Lie space) for sm_100a.
+// solver.cu -- sparse bundle adjustment (Gauss-Newton + Jacobi-PCG in Lie space) for sm_90a.
 // Implements include/bf_solver.h (rows a10-a12, a14-a16 of SURVEY.md section 8).
 //
 // Behavioural source: FL/Solver/SolverBundling.cu:756-1264, FL/Solver/SolverBundlingEquationsLie.h:27-228,
 // FL/Solver/LieDerivUtil.h:19-307, FL/SBA.cu:75-119.
 //
-// B200-first design (DESIGN.md section "Solver"):
+// Design (DESIGN.md section "Solver"):
 //  * the reference applies the sparse term matrix-free, J^T(J p), touching every correspondence twice per PCG
 //    iteration (~140 B/correspondence/iteration) and needs ~9 launches + a blocking device->host copy per
 //    iteration.  Here the correspondences of one image pair are folded ONCE per Gauss-Newton iteration into a

@@ -1,4 +1,4 @@
-// trajectory.cu -- trajectory glue for sm_100a.  Implements include/bf_bundler.h (row a22 of SURVEY.md section 8).
+// trajectory.cu -- trajectory glue for sm_90a.  Implements include/bf_bundler.h (row a22 of SURVEY.md section 8).
 // Behavioural source (what, not how): FL/OnlineBundler.cu:6-140.  Tiny kernels; what matters is that they exist behind the
 // reference's stub names, run on the library stream without a host synchronisation, and agree bit for bit with
 // oracle/trajectory_oracle.c (this TU is built -fmad=false; products are fused only as mat4.cuh writes them).

@@ -1,10 +1,10 @@
 // tsdf.cu -- hashed-voxel TSDF: reset / alloc / compactify / integrate / de-integrate / GC
-// for sm_100a.  Implements include/bf_tsdf.h (rows a1-a9 of SURVEY.md section 8).
+// for sm_90a.  Implements include/bf_tsdf.h (rows a1-a9 of SURVEY.md section 8).
 //
 // Behavioural source (what, not how): FL/DepthSensing/CUDASceneRepHashSDF.cu:27-684,
 // FL/DepthSensing/VoxelUtilHashSDF.h:226-826, FL/DepthSensing/DepthCameraUtil.h:71-144.
 //
-// B200-first design (see DESIGN.md section "TSDF"):
+// Design (see DESIGN.md section "TSDF"):
 //  * no __constant__ uploads, no texture binds: parameters travel as __grid_constant__
 //    kernel arguments, images are read through the read-only path;
 //  * allocation is ONE kernel (in-kernel bucket spin locks), not a host retry loop with a
@@ -1470,8 +1470,8 @@ static int ensure_tiles(TsdfAux* aux, const BFDepthCameraParams* cp) {
     aux->tilesCap = need;
     return 0;
 }
-// Per-block depth-range cull: OFF by default.  Measured on the bench stream (profiles/r1_tsdf_experiments.md): the cull test
-// lengthens the compactify kernels' critical path by ~4.5 us per call while the blocks it can prove dead (mostly: looking at
+// Per-block depth-range cull: OFF by default.  The cull test lengthens the compactify kernels' critical path on every call while the
+// blocks it can prove dead (mostly: looking at
 // depths beyond the integration distance) were cheap for the stencil anyway (their probes exit at the depth test).
 // bfTsdfSetBlockCull(1) or BF_TSDF_CULL=1 switches it on; results are identical either way (tests/test_tsdf_gpu.py).
 static int g_lanes = -1;             // two-lane op replay (bfTsdfRunOps), see "two lanes" below
@@ -1566,9 +1566,8 @@ static int stencil_end(TsdfAux* aux) {
     if (aux->pipeOpen) { BF_CHECK(cudaEventRecord(aux->evStencil[aux->parity], aux->lane)); aux->stencilPending[aux->parity] = true; }
     return 0;
 }
-// Stencil CTAs per SM inside a two-lane bracket.  Measured (profiles/r1_tsdf_experiments.md section 5): capping the stencil at 4-6
-// CTAs per SM so that alloc CTAs can co-reside costs the stencil more (38 -> 49-60 us) than the overlap returns; uncapped, the
-// front lane fills the SMs the stencil's last wave frees, worth ~7 % of the TSDF time.
+// Stencil CTAs per SM inside a two-lane bracket.  Capping the stencil at 4-6 CTAs per SM so that alloc CTAs can co-reside slows the
+// stencil by more than the overlap returns; uncapped, the front lane fills the SMs the stencil's last wave frees.
 static int stencil_per_sm() {
     static int v = -1;
     if (v < 0) { const char* e = getenv("BF_TSDF_LANE_STENCIL_PER_SM"); v = e ? atoi(e) : 16; if (v < 1) v = 1; if (v > 16) v = 16; }

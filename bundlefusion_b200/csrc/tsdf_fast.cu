@@ -4,8 +4,8 @@
 // DepthCameraUtil.h:71-82 (projection), the re-integration loop of FL/DepthSensing/DepthSensing.cpp:854-902.
 //
 // Why a second stencil.  tsdf.cu reproduces the reference's IEEE build bit for bit (individually rounded operations, two IEEE
-// divides per voxel probe, the full 4x4 product per voxel): ~130 thread-instructions per probe, issue-bound at 18 % of the HBM
-// roof on the re-integration stream (profiles/r1_ncu_full_reintegrate_alloc.txt).  The reference itself ships --use_fast_math
+// divides per voxel probe, the full 4x4 product per voxel): ~130 thread-instructions per probe, issue-bound far below the HBM
+// roof on the re-integration stream.  The reference itself ships --use_fast_math
 // and BASELINE's north star asks for "weights/sdf within a stated fp32 tolerance", so the product path is this one:
 //   * the voxel -> camera transform is affine in the integer voxel coordinate: one FMA chain per (thread, block) and three adds
 //     per further x-consecutive voxel instead of a 4x4 product per voxel;
@@ -17,7 +17,7 @@
 // Contract (tests/test_tsdf_fast_gpu.py): allocated block set identical (alloc / compactify stay in tsdf.cu), weights identical,
 // |d sdf| <= 1e-5 m, colour +-1, except for a <= 1e-4 fraction of voxels whose projected pixel or truncation test sits within
 // rounding distance of its decision boundary -- the same kind and size of difference the reference's own --use_fast_math build
-// shows against its IEEE build (profiles/r1_tsdf_parity_vs_reference_cuda.txt).  bfTsdfSetArithmetic(BF_TSDF_ARITH_EXACT)
+// shows against its IEEE build (tests/test_tsdf_vs_reference_gpu.py).  bfTsdfSetArithmetic(BF_TSDF_ARITH_EXACT)
 // selects tsdf.cu's kernels.
 #include "bf_common.cuh"
 #include "tsdf_shared.cuh"

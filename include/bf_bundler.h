@@ -28,7 +28,7 @@ void updateTrajectoryCU(const float* d_globalTrajectory, unsigned int numGlobalT
                         const float* d_localTrajectories, unsigned int numLocalTransformsPerTrajectory, unsigned int numLocalTrajectories,
                         int* d_imageInvalidateList);
 
-/* ---- B200-native extension: the re-integration choice of TrajectoryManager::generateUpdateLists (FL/TrajectoryManager.cpp:45-108) on
+/* ---- H100-native extension: the re-integration choice of TrajectoryManager::generateUpdateLists (FL/TrajectoryManager.cpp:45-108) on
  * the device.  The reference copies the whole optimised trajectory to the host every frame, converts every pose with MatrixToPose, and
  * std::sorts all frames to take the top N.  Here one launch computes, per frame, dist = |(s t, w)_integrated - (s t, w)_optimised|^2
  * ((w, t) = the SE(3) logarithm, s = rescaleRotToTrans = 2: despite its name the factor multiplies the TRANSLATION part -- the host's

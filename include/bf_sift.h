@@ -158,8 +158,7 @@ int bfSiftCheckForInvalidFrames(const int32_t* d_varToCorrNumEntriesPerRow, int3
  * *d_numKeyPoints (DEVICE counter: the reference copies its level counts to the host mid-way, this path never leaves the device),
  * d_levelCounts: optional device int[12], features per (octave, level).  width must be a multiple of 32, height of 8, both >= 64.
  * Differences from the reference (its lists are appended with atomicAdd): key points of a level come in raster order, an orientation
- * pair as (first, second); histogram sums are taken in scheduling order here as there.  Asynchronous on the library stream.
- * STATUS: compiled for sm_100a, not yet run on hardware (see csrc/sift_detect.cu). */
+ * pair as (first, second); histogram sums are taken in scheduling order here as there.  Asynchronous on the library stream. */
 typedef struct BFSiftDetectParams {
     uint32_t width, height;              /* SIFT (intensity) image */
     uint32_t depthWidth, depthHeight;

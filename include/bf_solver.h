@@ -18,7 +18,7 @@
  * private block-sparse workspace per BFSolverState (keyed by d_deltaRot), created on first use; d_denseJtJ
  * (the reference's dense (6N)^2 matrix), d_Jp, d_zRot/d_zTrans and d_Ap_* are accepted but not needed.
  *
- * Part 2 (bfSolver*) is the sync-free B200 entry: one call = one whole CUDASolverBundling::solve, all GN
+ * Part 2 (bfSolver*) is the sync-free entry: one call = one whole CUDASolverBundling::solve, all GN
  * iterations and PCG iterations on the device, early-outs evaluated on the device, no device->host copy.
  */
 #ifndef BF_SOLVER_H
@@ -157,7 +157,7 @@ void convertMatricesToPosesCU(const float* d_transforms, unsigned int numTransfo
 void convertPosesToMatricesCU(const float* d_rot, const float* d_trans, unsigned int numImages, float* d_transforms,
                               const int* d_validImages);
 
-/* ---------------- Part 2: B200-native extension ---------------- */
+/* ---------------- Part 2: H100-native extension ---------------- */
 
 /* One whole solve, asynchronous on the library stream.  weights*: HOST arrays of nNonLinearIterations entries
  * (copied into the launch).  Returns 0 or a cudaError_t. */

@@ -21,7 +21,7 @@
  * see below and SURVEY.md quirk Q1).  Types carry a BF prefix so that both headers can be
  * visible in one translation unit.
  *
- * The second half (bfTsdf*) is the B200-native, sync-free extension the host
+ * The second half (bfTsdf*) is the H100-native, sync-free extension the host
  * mirror class (bundlefusion_b200/host/SceneRepHashSDF.h) drives: one call per
  * integrate / de-integrate, no device->host copy, no constant upload.
  *
@@ -180,7 +180,7 @@ void garbageCollectIdentifyCUDA(BFHashDataStruct* hashData, const BFHashParams* 
 void garbageCollectFreeCUDA(BFHashDataStruct* hashData, const BFHashParams* hashParams);
 
 /* ------------------------------------------------------------------------ *
- *  Part 2: B200-native extension (what the host mirror class calls).       *
+ *  Part 2: H100-native extension (what the host mirror class calls).       *
  *  All calls are asynchronous on the stream set by bfSetStream(); they      *
  *  return 0 or a cudaError_t value and never terminate the process.         *
  * ------------------------------------------------------------------------ */

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Builds oracle/_ref/: the REFERENCE's own TSDF kernels, compiled for sm_100a from the sources where they lie under
+"""Builds oracle/_ref/: the REFERENCE's own TSDF kernels, compiled for sm_90a from the sources where they lie under
 /root/reference, with a mechanical, behaviour-preserving compatibility patch applied to a scratch copy (the reference does
 not compile under CUDA 12.9 as it is, SURVEY.md section 8c).  Nothing from the reference is copied into the repository; the
 outputs are shared libraries under oracle/_ref/ (git-ignored, shipped to the GPU box by gpurun).
@@ -84,7 +84,7 @@ def main():
     patch(os.path.join(TMP, "DepthCameraUtil.h"), [(r"extern __constant__ DepthCameraParams c_depthCameraParams;", "", 1)])
     open(unit, "w").write('#include "CUDAConstant.cu"\n#include "CUDASceneRepHashSDF.cu"\n')
     inc = ["-I", TMP, "-I", os.path.join(REF, "Include", "cutil", "inc")]
-    base = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-w", "-shared", "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic",
+    base = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-w", "-shared", "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic",
             "-Xcompiler", "-fpermissive"] + inc
     for name, extra in (("libref_tsdf_fast.so", ["--use_fast_math"]), ("libref_tsdf.so", [])):
         cmd = base + extra + [unit, "-o", os.path.join(OUT, name), "-lcudart"]
@@ -108,7 +108,7 @@ def main():
 
 
 def build_solver():
-    """The reference's bundle-adjustment solver (FL/Solver/SolverBundling.cu + FL/SBA.cu) for sm_100a -> libref_solver[_fast].so.
+    """The reference's bundle-adjustment solver (FL/Solver/SolverBundling.cu + FL/SBA.cu) for sm_90a -> libref_solver[_fast].so.
     Scratch tree mirrors the reference's relative include layout; patches: the two listed at the top (template<>, shfl_sync) plus
       5. FL/Solver/SolverBundlingUtil.h : `__shfl_down` -> `_sync`;
       6. FL/SBA.cu : the Windows back-slash in the LieDerivUtil.h include -> slash;
@@ -141,7 +141,7 @@ def build_solver():
     open(os.path.join(st, "core-base", "common.h"), "w").write(
         "#pragma once\n#include <stdexcept>\n#include <string>\n#define MLIB_EXCEPTION(s) std::runtime_error(std::string(s))\n"
         "#define MLIB_ASSERT(x)\n#define SAFE_DELETE_ARRAY(p) { if (p) { delete[] (p); (p) = NULL; } }\n")
-    base = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-w", "-shared", "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic",
+    base = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-w", "-shared", "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic",
             "-Xcompiler", "-fpermissive", "-I", st, "-I", src, "-I", os.path.join(src, "SiftGPU"), "-I", os.path.join(src, "Solver"),
             "-I", os.path.join(REF, "Include", "cutil", "inc")]
     for name, extra in (("libref_solver_fast.so", ["--use_fast_math"]), ("libref_solver.so", [])):
@@ -154,7 +154,7 @@ def build_solver():
 
 def build_siftmgr():
     """The reference's match-manager kernels (FL/SiftGPU/SIFTImageManager.cu: SortKeyPointMatchesCU, FilterKeyPointMatchesCU,
-    FilterMatchesBySurfaceAreaCU, FilterMatchesByDenseVerifyCU, AddCurrToResidualsCU) for sm_100a -> libref_siftmgr[_fast].so, through
+    FilterMatchesBySurfaceAreaCU, FilterMatchesByDenseVerifyCU, AddCurrToResidualsCU) for sm_90a -> libref_siftmgr[_fast].so, through
     oracle/ref_siftmgr_wrap.cu (our own C entry points, which includes the scratch copy as one translation unit).  Patches: template<>
     and shfl_sync as above, in every header that uses them; stub headers as for the solver."""
     root = os.path.join(TMP, "siftmgr")
@@ -178,7 +178,7 @@ def build_siftmgr():
     open(os.path.join(st, "core-base", "common.h"), "w").write(
         "#pragma once\n#include <stdexcept>\n#include <string>\ntypedef unsigned char uchar;\n#define MLIB_EXCEPTION(s) std::runtime_error(std::string(s))\n"
         "#define MLIB_ASSERT(x)\n#define SAFE_DELETE_ARRAY(p) { if (p) { delete[] (p); (p) = NULL; } }\n")
-    base = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-w", "-shared", "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic",
+    base = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-w", "-shared", "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic",
             "-Xcompiler", "-fpermissive", "-I", st, "-I", src, "-I", sg, "-I", os.path.join(REF, "Include", "cutil", "inc")]
     for name, extra in (("libref_siftmgr_fast.so", ["--use_fast_math"]), ("libref_siftmgr.so", [])):
         cmd = base + extra + [os.path.join(HERE, "ref_siftmgr_wrap.cu"), "-o", os.path.join(OUT, name), "-lcudart"]

@@ -7,7 +7,7 @@
  * by the known-answer tests in tests/test_solver_oracle.py (SE(3) exp/log identities, recovery of known poses
  * from exact correspondences, agreement with an independent float64 dense Gauss-Newton written in numpy,
  * finite-difference rows of the dense Jacobian) AND by tests/golden/solver_reference_ieee.npz: poses solved by the reference's
- * own SolverBundling.cu (oracle/_ref, run on a B200 by scripts/make_golden_from_reference.py) for a sparse 11-image problem and a
+ * own SolverBundling.cu (oracle/_ref, run on a GPU by scripts/make_golden_from_reference.py) for a sparse 11-image problem and a
  * sparse + dense 5-image problem, which tests/test_golden_reference.py requires this oracle to reproduce within 1e-4 relative L2
  * (and the dense overlap count exactly).  On the GPU box it is additionally pinned against the reference live:
  * tests/test_solver_vs_reference_gpu.py runs the reference's own SolverBundling.cu / SBA.cu (oracle/_ref, built

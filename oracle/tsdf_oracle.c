@@ -9,8 +9,8 @@
  * PARITY STATUS: PINNED against the reference itself.  The reference ships no golden vectors or tests for this path (SURVEY.md
  * section 4 / 8c) and its .cu files neither compile with CUDA 12.9 as they are nor run without a GPU, so the pin is made of
  * (a) tests/golden/tsdf_reference_ieee.npz -- outputs of the reference's OWN kernels (oracle/_ref: CUDASceneRepHashSDF.cu built
- *     for sm_100a from /root/reference with the mechanical compat patch of oracle/build_ref.py, IEEE build) on a seeded stream
- *     (3 integrations, a re-integration, GC), produced on a B200 by scripts/make_golden_from_reference.py and replayed through
+ *     for sm_90a from /root/reference with the mechanical compat patch of oracle/build_ref.py, IEEE build) on a seeded stream
+ *     (3 integrations, a re-integration, GC), produced on a GPU by scripts/make_golden_from_reference.py and replayed through
  *     this file by tests/test_golden_reference.py in the CPU-only suite: block set, heap count and EVERY voxel word bit-identical;
  * (b) tests/test_tsdf_vs_reference_gpu.py on the GPU box (this oracle's contract = the CUDA library = the reference's kernels);
  * (c) analytic known-answer tests we author (tests/test_tsdf_oracle.py).

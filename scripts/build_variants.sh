@@ -6,10 +6,10 @@ cd "$(dirname "$0")/.."
 mkdir -p build_variants
 make -s -C bundlefusion_b200/csrc >/dev/null 2>&1
 C=bundlefusion_b200/csrc
-FLAGS="-O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-fvisibility=hidden -gencode arch=compute_100a,code=sm_100a -fmad=false -prec-div=true -prec-sqrt=true"
+FLAGS="-O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-fvisibility=hidden -gencode arch=compute_90a,code=sm_90a -fmad=false -prec-div=true -prec-sqrt=true"
 for spec in "$@"; do
   name="${spec%%:*}"; defs="${spec#*:}"
   nvcc $FLAGS $defs -c $C/tsdf.cu -o build_variants/tsdf_$name.o
-  nvcc -shared -gencode arch=compute_100a,code=sm_100a -o build_variants/lib_$name.so build_variants/tsdf_$name.o $C/host_api.o $C/solver.o -lcudart
+  nvcc -shared -gencode arch=compute_90a,code=sm_90a -o build_variants/lib_$name.so build_variants/tsdf_$name.o $C/host_api.o $C/solver.o -lcudart
   echo "built build_variants/lib_$name.so  ($defs)"
 done

@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
 
 
 # Collection order of the GPU tests (the driver runs `pytest -x`): the voxel-hash tests first, then the other rows against the oracle,
-# then the comparisons with the reference's own CUDA build (they depend on oracle/_ref and on the reference's non-deterministic float
-# atomics), last the kernels with the shortest hardware history.  One failure must hide as little verified work as possible.
+# then the comparisons with the recorded outputs of the reference's own CUDA build (tests/reference_cuda.py), last the kernels with the
+# shortest hardware history.  One failure must hide as little verified work as possible.
 _ORDER = {"test_tsdf_gpu.py": 0, "test_tsdf_vs_reference_gpu.py": 1, "test_solver_vs_reference_gpu.py": 5,
           "test_zz_sift_prune_gpu.py": 6, "test_zz_sift_detect_gpu.py": 7, "test_marchingcubes_gpu.py": 8, "test_sens_frame_loop_gpu.py": 9, "test_zz_scan_to_mesh_gpu.py": 10}          # 8 - 10: written after the round's last GPU minute -- first hardware run is the driver's
 

@@ -1,5 +1,5 @@
 """The match-filter kernels (csrc/sift_filter.cu, csrc/sift_verify.cu) under the CPU emulation of tests/cuda_emu, against the oracle.
-These kernels ARE verified on the B200 (tests/test_filter_gpu.py, tests/test_verify_filters_gpu.py: bit-identical to the oracle); running
+These kernels ARE verified on the GPU (tests/test_filter_gpu.py, tests/test_verify_filters_gpu.py: bit-identical to the oracle); running
 the same sources through the emulation and getting the same bits is what qualifies the emulation as a checker for the kernels that
 have not been on hardware yet (tests/test_sift_detect_emulated.py, tests/test_sift_prune_emulated.py)."""
 import ctypes as C

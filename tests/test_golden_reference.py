@@ -1,4 +1,4 @@
-"""The CPU oracle against committed outputs of the REFERENCE'S OWN CUDA (tests/golden/*.npz, produced on a B200 by
+"""The CPU oracle against committed outputs of the REFERENCE'S OWN CUDA (tests/golden/*.npz, produced on a GPU by
 scripts/make_golden_from_reference.py from oracle/_ref's IEEE build of CUDASceneRepHashSDF.cu / SolverBundling.cu): the same seeded inputs
 are regenerated here and replayed through oracle/*.c.  This is the pin of the oracle that runs without a GPU.
 TSDF: allocated block set, heap count and every voxel word (CRC per block) bit-identical to the reference's kernels.
@@ -26,7 +26,7 @@ def _load(name):
 
 def _inverse_subdeterminants(T):
     """The 4x4 inverse through 2x2 sub-determinants, float32, each operation rounded: how the pose inverses handed to the reference's kernels were formed when
-    tsdf_reference_ieee.npz was generated on the B200 (round 1).  The library now forms them as the reference's host does (tests/test_mat4_inverse_reference.py); the
+    tsdf_reference_ieee.npz was generated on a GPU (round 1).  The library now forms them as the reference's host does (tests/test_mat4_inverse_reference.py); the
     kernels' parity does not depend on which inverse they are handed, the stored voxel words do -- so this test hands the oracle the inverses the generator used."""
     f = np.float32
     a = [f(x) for x in np.asarray(T, F).reshape(16)]

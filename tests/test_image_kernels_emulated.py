@@ -1,5 +1,5 @@
 """The dense-cache, frame-ingest and trajectory kernels (csrc/cache.cu, csrc/ingest.cu, csrc/trajectory.cu) under the CPU emulation of
-tests/cuda_emu, against the oracle, bit for bit.  These kernels are verified on the B200 (tests/test_cache_gpu.py, test_ingest_gpu.py,
+tests/cuda_emu, against the oracle, bit for bit.  These kernels are verified on the GPU (tests/test_cache_gpu.py, test_ingest_gpu.py,
 test_trajectory_gpu.py); the emulated runs keep them covered when no GPU is at hand and qualify the emulation a second time."""
 import ctypes as C
 
@@ -81,7 +81,7 @@ def test_trajectory_kernels_emulated(libs):
 
 
 def test_select_reintegration_emulated(libs):
-    """bfTrajectorySelectReintegration (verified on the B200 before the scaled component of the pose distance was corrected to the translation
+    """bfTrajectorySelectReintegration (verified on the GPU before the scaled component of the pose distance was corrected to the translation
     part, FL/TrajectoryManager.cpp:67-74): the kernel against the oracle under the emulation."""
     Lt = libs[2]
     from tests.test_manager_reference_emulated import poses

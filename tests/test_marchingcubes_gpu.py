@@ -61,6 +61,7 @@ def test_marching_cubes_matches_oracle_bit_for_bit(cuda_device, tmp_path):
     # saveMesh: merge / de-duplicate / PLY; an existing file is kept and the name counts up; the buffer is cleared
     mc.clearMeshBuffer()
     mc.extractIsoSurface(gpu)
+    soup_pos, soup_col = mc.soup()
     path = str(tmp_path / "scans" / "scan.ply")
     first = mc.saveMesh(path)
     assert first == path and os.path.exists(path) and mc.soup()[0].shape[0] == 0
@@ -80,7 +81,19 @@ def test_marching_cubes_matches_oracle_bit_for_bit(cuda_device, tmp_path):
     v2, f2 = read_ply(second)
     # the merged mesh: every cell edge vertex once instead of once per adjoining triangle; (almost) every triangle survives
     assert len(v1) < len(want) and 0.98 * len(want) < len(f1) <= len(want) and f1["i"].max() <= len(v1) - 1 and f1["i"].min() == 0
-    assert len(v2) == len(v1) and np.allclose(v2["p"], 2.0 * v1["p"], rtol=1e-6, atol=0) and np.array_equal(v2["c"], v1["c"])
+    # the two extractions append their triangles in scheduling order, so the files list their vertices in different orders, and which member of a
+    # group of vertices closer than the merge threshold (1e-5) represents the group -- position and colour -- can differ (the members are one edge point
+    # seen from adjacent cells, coloured from different voxels): every vertex of the second file is a vertex of the first scaled by 2, to within twice the
+    # threshold per axis, each vertex of the first is matched once, and where the two colours differ each is the colour of a member of that group
+    from scipy.spatial import cKDTree
+    dist, nn = cKDTree(2.0 * v1["p"].astype(np.float64)).query(v2["p"].astype(np.float64), p=np.inf)
+    assert len(v2) == len(v1) and dist.max() <= 2 * 2e-5 and len(np.unique(nn)) == len(v1)
+    soup_u8 = (soup_col * np.float32(255)).astype(np.uint8)                  # the PLY writer's (uchar)(colour * 255)
+    differ = np.flatnonzero(np.any(v2["c"] != v1["c"][nn], axis=1))
+    groups = cKDTree(soup_pos.astype(np.float64)).query_ball_point(v1["p"][nn[differ]].astype(np.float64), r=2 * 2e-5, p=np.inf)
+    for i, members in zip(differ, groups):
+        seen = {c.tobytes() for c in soup_u8[members]}
+        assert v1["c"][nn[i]].tobytes() in seen and v2["c"][i].tobytes() in seen, (i, v1["c"][nn[i]], v2["c"][i])
     mc.close(); gpu.close()
 
 

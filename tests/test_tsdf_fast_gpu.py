@@ -6,8 +6,7 @@ Contract (include/bf_tsdf.h, bfTsdfSetArithmetic):
 * allocated block set, in-frustum list, heap count: identical (allocation and list building do not change with the arithmetic);
 * weights identical, |d sdf| <= 1e-5 m, colour within 1 level -- for all voxels but a counted fraction <= 1e-4 whose projected pixel or
   truncation test sits within float rounding distance of its decision boundary (such a voxel samples the neighbouring depth pixel, or is
-  / is not updated: weight differs by one).  The reference's own fast-math build differs from its IEEE build in the same way
-  (profiles/r1_tsdf_parity_vs_reference_cuda.txt: 1.1e-5 flips, 5e-7 weight mismatches)."""
+  / is not updated: weight differs by one).  The reference's own fast-math build differs from its IEEE build in the same way."""
 import numpy as np
 import pytest
 
@@ -15,8 +14,7 @@ from bundlefusion_b200 import _capi as capi
 from bundlefusion_b200 import synth
 from bundlefusion_b200.scene_rep import CUDASceneRepHashSDF, camera_params, default_hash_params
 from oracle import oracle as orc
-from oracle import ref_tsdf
-from tests.test_tsdf_vs_reference_gpu import compare_states
+from tests.test_tsdf_vs_reference_gpu import compare_states, reference_stream, reintegration_pose
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -91,31 +89,27 @@ def test_fast_fused_reintegration_matches_oracle_and_exact_kernels(cuda_device):
 
 @pytest.mark.parametrize("fast_math", [False, True])
 def test_fast_stream_matches_reference_cuda(cuda_device, fast_math):
-    """the same statement against the reference's own CUDA kernels (oracle/_ref), IEEE build and --use_fast_math build"""
+    """the same statement against the reference's own CUDA kernels (oracle/_ref, recorded: tests/golden/tsdf_reference_cuda.npz), IEEE build
+    and --use_fast_math build"""
     import torch
-    if not ref_tsdf.available(fast_math):
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
     W, H = 320, 240
     cam = camera_params(W, H)
     hp = default_hash_params(num_buckets=100003, num_sdf_blocks=60000)
     ours = CUDASceneRepHashSDF(hp, cuda_device, arithmetic="fast")
-    ref = ref_tsdf.ReferenceSceneRepHashSDF(hp, cuda_device, fast_math=fast_math)
     frames, dl, cl = _frames(torch, cuda_device, 6, W, H)
+    ref1, ref2, n = reference_stream(cuda_device, hp, cam, frames, fast_math)
     tol = 1e-4 if fast_math else SDF_TOL          # the reference's fast-math build is itself ~1e-5 away from IEEE
     for (d, c, T), dd, dc in zip(frames, dl, cl):
         ours.integrate(T, dd, dc, cam)
-        ref.integrate(T, dd, dc, cam)
-    s1 = compare_states(ours.download(), ref.download(), tol)
-    assert ours.getNumOccupiedBlocks() == ref.hp.m_numOccupiedBlocks and ours.getHeapFreeCount() == ref.getHeapFreeCount()
+    s1 = compare_states(ours.download(), ref1, tol)
+    assert ours.getNumOccupiedBlocks() == n["occupied1"] and ours.getHeapFreeCount() == n["free1"]
     for k in (1, 4):
         d, c, T = frames[k]
-        T2 = T.copy(); T2[:3, 3] += np.array([0.011, -0.006, 0.004], F)
-        ours.runOps([(capi.BF_TSDF_OP_DEINTEGRATE, k, T), (capi.BF_TSDF_OP_INTEGRATE, k, T2)], dl, cl, cam)       # fused pass
-        ref.deIntegrate(T, dl[k], cl[k], cam); ref.integrate(T2, dl[k], cl[k], cam)
-    ours.deIntegrate(frames[0][2], dl[0], cl[0], cam); ref.deIntegrate(frames[0][2], dl[0], cl[0], cam)
-    ours.garbageCollect(); ref.garbageCollect()
-    s2 = compare_states(ours.download(), ref.download(), 10 * tol)
-    assert ours.getHeapFreeCount() == ref.getHeapFreeCount()
+        ours.runOps([(capi.BF_TSDF_OP_DEINTEGRATE, k, T), (capi.BF_TSDF_OP_INTEGRATE, k, reintegration_pose(T))], dl, cl, cam)       # fused pass
+    ours.deIntegrate(frames[0][2], dl[0], cl[0], cam)
+    ours.garbageCollect()
+    s2 = compare_states(ours.download(), ref2, 10 * tol)
+    assert ours.getHeapFreeCount() == n["free2"]
     print("fast vs reference CUDA (fast_math=%s):" % fast_math, s1, s2)
 
 
