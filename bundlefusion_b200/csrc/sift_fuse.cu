@@ -6,10 +6,12 @@
 // recursively into tracks, averages each track's world position, projects it into the chunk's first frame and uploads the fused key points
 // with one representative descriptor each as the next keyframe of the global manager.
 //
-// Here the whole thing is one launch of one CTA and nothing leaves the device: the lists are built in shared memory, all threads pick out the keys
-// that have correspondences at all, ONE thread replays the reference's recursion over those with an explicit stack (the visiting order decides which
-// key represents a track and which correspondence supplies a member's position, so it is reproduced, not parallelised: <= 1 375 correspondences per
-// chunk), then the tracks are reduced, compacted and their descriptors gathered by all threads.  Output and count stay on the device for the global matcher.
+// Here the whole thing is one launch of one CTA and nothing leaves the device, and every phase runs on all threads.  The lists are filled in
+// shared memory and sorted into push order; connected components of the key / correspondence graph are labelled; the reference's serial walk
+// over all roots equals one walk per component that holds a root, in the order of its first root, so each such component's walk is replayed
+// by one thread with an explicit stack, into its own slot of the track list (the visiting order decides which key represents a track and which
+// correspondence supplies a member's position, so it is reproduced exactly).  A walk's stack is sized by its component, so d_status (stack
+// overflow) cannot be raised.  Then the tracks are reduced, compacted and their descriptors gathered.  Output and count stay on the device.
 // Arithmetic as the reference's host code: individually rounded IEEE operations (this TU is built -fmad=false -prec-div=true -prec-sqrt=true),
 // float4x4 * float3 as ((m0 x + m1 y) + m2 z) + m3.  Bit-identical to oracle/fuse_oracle.c.
 #include "../../include/bf_sift.h"
@@ -21,7 +23,6 @@ extern unsigned long long g_launchCount;
 
 #define FUSE_MAX_KEYS 16384u       // numImages * keyStride
 #define FUSE_MAX_CORR 4096u
-#define FUSE_STACK 4096u
 #define FUSE_THREADS 1024
 
 struct FuseArgs {
@@ -46,15 +47,15 @@ sift_fuse_kernel(const __grid_constant__ FuseArgs a) {
     unsigned* adjCE = adjKey + 2 * C;             // [2C]      correspondence * 2 + side (0: target is the j side, 1: the i side)
     unsigned* trackItem = adjCE + 2 * C;          // [2C]      list entries in visiting order
     unsigned* trackStart = trackItem + 2 * C;     // [C + 1]
-    unsigned* stackKey = trackStart + (C + 1);    // [FUSE_STACK]
-    unsigned* stackPos = stackKey + FUSE_STACK;   // [FUSE_STACK]
-    unsigned* scan = stackPos + FUSE_STACK;       // [FUSE_THREADS]
+    unsigned* label = trackStart + (C + 1);       // [2C]      component label of a key's list-begin node
+    unsigned* comp = label + 2 * C;               // [C]       root of each track
+    unsigned* scan = comp + C;                    // [FUSE_THREADS]
     unsigned* rootList = scan + FUSE_THREADS;     // [2C]      keys with a non-empty list, in (image, key) order: the only roots that can start a track
     unsigned* ckx = rootList + 2 * C;             // [C]       key of the correspondence in image i (0xFFFFFFFF: invalid correspondence) ...
-    unsigned* cky = ckx + C;                      // [C]       ... and in image j: staged by all threads so that the serial list fill reads shared memory only
+    unsigned* cky = ckx + C;                      // [C]       ... and in image j
     unsigned char* marker = reinterpret_cast<unsigned char*>(cky + C);                   // [M]
     unsigned char* errOk = marker + ((M + 3) & ~3u);                                      // [C]
-    __shared__ unsigned sNumTracks, sOverflow, sNumRoots, sTotal;
+    __shared__ unsigned sNumTracks, sOverflow, sNumRoots, sTotal, sChanged;
 
     for (unsigned k = t; k <= M; k += FUSE_THREADS) start[k] = 0;
     for (unsigned k = t; k < M; k += FUSE_THREADS) marker[k] = 0;
@@ -94,21 +95,54 @@ sift_fuse_kernel(const __grid_constant__ FuseArgs a) {
         for (unsigned q = 0; q < per; ++q) { const unsigned k = 1 + t * per + q; if (k <= M) { const unsigned len = start[k]; start[k] = run + len; run += len; } }
         __syncthreads();           // now start[k + 1] = end of key k's list, start[0] = 0  => start[k] = begin of key k
     }
-    if (t == 0) {
-        // After the scan start[k] = begin of key k's list (= end of key k - 1's), start[M] = total.  The lists must be in push order =
-        // ascending correspondence index (:389-399).  Fill back to front: walking the correspondences in DESCENDING order and pre-decrementing
-        // the END pointer of the key (start[key + 1]) leaves every list ascending and turns start[key + 1] into the BEGIN of key's list;
-        // its end is then the begin of the next key's list, start[key + 2] (the total for the last key).
-        const unsigned total = start[M];
-        sTotal = total;                                  // start[M] is about to become the begin of the last key's list
-        for (int c = (int)C - 1; c >= 0; --c) {
-            const unsigned kx = ckx[c], ky = cky[c];
-            if (kx == 0xFFFFFFFFu) continue;
-            const unsigned sy = --start[ky + 1]; adjKey[sy] = kx; adjCE[sy] = 2u * (unsigned)c + 1u;
-            const unsigned sx = --start[kx + 1]; adjKey[sx] = ky; adjCE[sx] = 2u * (unsigned)c;
-        }
+    // After the scan start[k] = begin of key k's list (= end of key k - 1's), start[M] = total.  Pre-decrementing the END pointer of
+    // a key (start[key + 1]) for each of its entries turns it into the BEGIN of key's list; its end is then the begin of the next
+    // key's list, start[key + 2] (the total for the last key).  The lists must be in push order = ascending correspondence index,
+    // the i side before the j side (:389-399): entries land in any order, then every list is sorted by adjCE.
+    if (t == 0) sTotal = start[M];                   // start[M] is about to become the begin of the last key's list
+    __syncthreads();
+    for (unsigned c = t; c < C; c += FUSE_THREADS) {
+        const unsigned kx = ckx[c], ky = cky[c];
+        if (kx == 0xFFFFFFFFu) continue;
+        adjCE[atomicAdd(&start[ky + 1], 0xFFFFFFFFu) - 1u] = 2u * c + 1u;
+        adjCE[atomicAdd(&start[kx + 1], 0xFFFFFFFFu) - 1u] = 2u * c;
     }
     __syncthreads();
+    const unsigned total = sTotal;
+    for (unsigned k = t; k < M; k += FUSE_THREADS) {
+        const unsigned b = start[k + 1], e = (k + 1 < M) ? start[k + 2] : total;
+        for (unsigned i = b + 1; i < e; ++i) {                    // insertion sort: a list holds a few entries
+            const unsigned v = adjCE[i];
+            unsigned j = i;
+            for (; j > b && adjCE[j - 1] > v; --j) adjCE[j] = adjCE[j - 1];
+            adjCE[j] = v;
+        }
+        for (unsigned i = b; i < e; ++i) { const unsigned ce = adjCE[i]; adjKey[i] = (ce & 1u) ? ckx[ce >> 1] : cky[ce >> 1]; }
+    }
+    // Connected components of the key / correspondence graph.  A key with a non-empty list is named by its list's begin (node
+    // start[k + 1] < total, increasing with k); label[node] converges to the smallest node of its component by min-hooking and
+    // pointer jumping (label[x] <= x and in x's component throughout).
+    volatile unsigned* vlabel = label;                 // read while other threads lower it
+    for (unsigned i = t; i < total; i += FUSE_THREADS) label[i] = i;
+    for (;;) {
+        if (t == 0) sChanged = 0;
+        __syncthreads();
+        for (unsigned c = t; c < C; c += FUSE_THREADS) {
+            const unsigned kx = ckx[c], ky = cky[c];
+            if (kx == 0xFFFFFFFFu) continue;
+            const unsigned la = vlabel[start[kx + 1]], lb = vlabel[start[ky + 1]];
+            if (la != lb) { const unsigned m = min(la, lb); atomicMin(&label[la], m); atomicMin(&label[lb], m); sChanged = 1; }
+        }
+        __syncthreads();
+        for (unsigned i = t; i < total; i += FUSE_THREADS) {
+            unsigned p = vlabel[i];
+            for (unsigned pp = vlabel[p]; pp != p; pp = vlabel[p]) p = pp;
+            vlabel[i] = p;
+        }
+        const unsigned changed = sChanged;
+        __syncthreads();
+        if (!changed) break;
+    }
     // findTrack is called for every key in (image, key) order (:401-410), but a key without correspondences starts and joins nothing: all threads pick
     // out, in that order, the keys whose list is not empty (of ~2 000 keys of a chunk a few hundred), so that the serial walk below touches only those
     {
@@ -142,41 +176,86 @@ sift_fuse_kernel(const __grid_constant__ FuseArgs a) {
         if (t == FUSE_THREADS - 1) sNumRoots = scan[t];
         __syncthreads();
     }
-    if (t == 0) {
-        // the recursion of findTrack replaced by an explicit stack, roots in the reference's order
-        const unsigned total = sTotal, nRoots = sNumRoots;
-        unsigned nItems = 0, nTracks = 0;
-        for (unsigned r = 0; r < nRoots; ++r) {
-            {
-                const unsigned root = rootList[r];
-                const unsigned first = nItems;
-                unsigned sp = 1;
-                stackKey[0] = root; stackPos[0] = start[root + 1];
-                while (sp) {
-                    const unsigned cur = stackKey[sp - 1];
-                    const unsigned end = (cur + 1 < M) ? start[cur + 2] : total;
-                    unsigned pos = stackPos[sp - 1];
-                    bool descended = false;
-                    while (pos < end) {
-                        const unsigned tgt = adjKey[pos];
-                        if (!marker[tgt]) {
-                            trackItem[nItems++] = pos;
-                            marker[tgt] = 1;
-                            stackPos[sp - 1] = pos + 1;
-                            if (sp >= FUSE_STACK) { sOverflow = 1; break; }
-                            stackKey[sp] = tgt; stackPos[sp] = start[tgt + 1]; ++sp;
-                            descended = true;
-                            break;
-                        }
-                        ++pos;
-                    }
-                    if (!descended) --sp;
-                }
-                if (nItems > first) trackStart[nTracks++] = first;
+    // The serial reference walks findTrack from every root in rootList order.  A walk from root r marks exactly r's component, so
+    // only the first root of each component opens a track, and that track is the component's walk, independent of the others.
+    // Tracks are therefore the components that hold a root, in the order of their first root, walked in parallel below.
+    {
+        unsigned* firstRoot = trackItem;                 // [total] per component label: smallest rootList index (trackItem is written by the walks only)
+        unsigned* compSize = ckx;                        // [total] (ckx, cky: 2C words, no longer needed) per component label: keys
+        const unsigned nRoots = sNumRoots;
+        for (unsigned i = t; i < total; i += FUSE_THREADS) { firstRoot[i] = 0xFFFFFFFFu; compSize[i] = 0; }
+        __syncthreads();
+        for (unsigned r = t; r < nRoots; r += FUSE_THREADS) atomicMin(&firstRoot[label[start[rootList[r] + 1]]], r);
+        for (unsigned k = t; k < M; k += FUSE_THREADS)
+            if (start[k + 1] < ((k + 1 < M) ? start[k + 2] : total)) atomicAdd(&compSize[label[start[k + 1]]], 1u);
+        __syncthreads();
+        // compaction of the first roots in rootList order: comp[track] = root, trackStart[track] = its component's size
+        const unsigned per = (nRoots + FUSE_THREADS - 1) / FUSE_THREADS;
+        unsigned local = 0;
+        for (unsigned q = 0; q < per; ++q) { const unsigned r = t * per + q; if (r < nRoots && firstRoot[label[start[rootList[r] + 1]]] == r) ++local; }
+        scan[t] = local;
+        __syncthreads();
+        for (unsigned off = 1; off < FUSE_THREADS; off <<= 1) {
+            const unsigned v = (t >= off) ? scan[t - off] : 0u;
+            __syncthreads();
+            scan[t] += v;
+            __syncthreads();
+        }
+        unsigned o = scan[t] - local;
+        for (unsigned q = 0; q < per; ++q) {
+            const unsigned r = t * per + q;
+            if (r < nRoots) {
+                const unsigned lab = label[start[rootList[r] + 1]];
+                if (firstRoot[lab] == r) { comp[o] = rootList[r]; trackStart[o] = compSize[lab]; ++o; }
             }
         }
-        trackStart[nTracks] = nItems;
-        sNumTracks = nTracks;
+        if (t == FUSE_THREADS - 1) sNumTracks = scan[t];
+        __syncthreads();
+        // exclusive scan of the component sizes: trackStart[track] = first item of the track, trackStart[nTracks] = items
+        const unsigned nT = sNumTracks, perT = (nT + FUSE_THREADS) / FUSE_THREADS;
+        local = 0;
+        for (unsigned q = 0; q < perT; ++q) { const unsigned i = t * perT + q; if (i < nT) local += trackStart[i]; }
+        scan[t] = local;
+        __syncthreads();
+        for (unsigned off = 1; off < FUSE_THREADS; off <<= 1) {
+            const unsigned v = (t >= off) ? scan[t - off] : 0u;
+            __syncthreads();
+            scan[t] += v;
+            __syncthreads();
+        }
+        unsigned run = scan[t] - local;
+        for (unsigned q = 0; q < perT; ++q) { const unsigned i = t * perT + q; if (i < nT) { const unsigned len = trackStart[i]; trackStart[i] = run; run += len; } }
+        if (t == FUSE_THREADS - 1) trackStart[nT] = scan[t];
+        __syncthreads();
+    }
+    // One thread per track: the recursion of findTrack replaced by an explicit stack of list positions.  Every push marks a key of
+    // the component, so a track of n keys is at most n + 1 deep: its stack lives at trackStart[track] + track of the pool
+    // (rootList, ckx, cky: 4C words >= items + tracks) and cannot overflow into the next one.
+    for (unsigned tr = t; tr < sNumTracks; tr += FUSE_THREADS) {
+        const unsigned root = comp[tr], first = trackStart[tr], depth = trackStart[tr + 1] - first + 1;
+        unsigned* stack = rootList + first + tr;
+        unsigned nItems = first, sp = 1;
+        stack[0] = start[root + 1];
+        while (sp) {
+            const unsigned cur = (sp == 1) ? root : adjKey[stack[sp - 2] - 1];      // the entry that descended to this level
+            const unsigned end = (cur + 1 < M) ? start[cur + 2] : total;
+            unsigned pos = stack[sp - 1];
+            bool descended = false;
+            while (pos < end) {
+                const unsigned tgt = adjKey[pos];
+                if (!marker[tgt]) {
+                    trackItem[nItems++] = pos;
+                    marker[tgt] = 1;
+                    stack[sp - 1] = pos + 1;
+                    if (sp >= depth) { sOverflow = 1; break; }
+                    stack[sp] = start[tgt + 1]; ++sp;
+                    descended = true;
+                    break;
+                }
+                ++pos;
+            }
+            if (!descended) --sp;
+        }
     }
     __syncthreads();
     const unsigned nTracks = sNumTracks;
@@ -245,7 +324,7 @@ BF_API int bfSiftFuseToGlobal(const BFEntryJ* d_corr, const uint32_t* d_corrKeyI
     a.keys = d_keyPoints; a.descs = d_descriptors; a.numKeys = d_numKeysPerImage; a.keyStride = keyStride;
     for (int k = 0; k < 16; ++k) a.K[k] = colorIntrinsics[k];
     a.outKeys = d_outKeyPoints; a.outDescs = d_outDescriptors; a.outNum = d_outNumKeys; a.maxKeys = maxKeys; a.status = d_status;
-    const size_t words = (size_t)(M + 1) + 10 * (size_t)maxCorr + (maxCorr + 1) + 2 * FUSE_STACK + FUSE_THREADS;
+    const size_t words = (size_t)(M + 1) + 13 * (size_t)maxCorr + (maxCorr + 1) + FUSE_THREADS;
     const size_t bytes = words * 4 + ((M + 3) & ~3u) + ((maxCorr + 3) & ~3u);
     static size_t attr = 0;
     if (bytes > attr) { BF_CHECK(cudaFuncSetAttribute(sift_fuse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes)); attr = bytes; }

@@ -10,7 +10,7 @@
 //    iteration.  Here the correspondences of one image pair are folded ONCE per Gauss-Newton iteration into a
 //    6x6 block (block-sparse J^T J, both (i,j) and (j,i) stored so a row never needs a transpose), and a PCG
 //    iteration is a block-sparse mat-vec over ~144 B per image pair -- ~25x less traffic, L2-resident;
-//  * one persistent cooperative kernel runs a whole Gauss-Newton iteration: pose -> matrix, block build, row
+//  * one persistent kernel (a cooperative grid; one CTA at small N) runs a whole Gauss-Newton iteration: pose -> matrix, block build, row
 //    reduction, PCG init, all PCG iterations (2 grid barriers each), Lie update, convergence test.  The early-outs
 //    (|p.Ap| < 5e-7, max|delta| < 0.005) are evaluated on the device; later GN launches see a "done" flag;
 //  * every floating-point reduction has a fixed shape (per-segment serial sums, fixed warp trees, partials summed
@@ -35,6 +35,7 @@ extern unsigned long long g_launchCount;      // defined in tsdf.cu (bfGetLaunch
 #define BF_MAX_ROW 8192                 // longest variable row the in-smem row sort handles
 #define BF_SOLVER_THREADS 256
 #define BF_SOLVER_MAX_PEERS 8
+#define BF_SOLVER_ONE_CTA_MAX_N 16u      // largest N whose Gauss-Newton iterations run as one CTA (OneCtaGrid)
 #define BF_DENSE_MAX_IMAGES 4096        // dense term: N^2 pair tables + one 90-sum record per image pair (allocated on first use, sized by the workspace)
 
 __device__ void mat4_mul(const float* a, const float* b, float* o) {
@@ -295,7 +296,7 @@ prep_rows_kernel(BFEntryJ* corr, const int* __restrict__ rowStart, int* entries,
     }
 }
 
-// ---- the Gauss-Newton iteration kernel (cooperative, persistent) ------------------------------------------------
+// ---- the Gauss-Newton iteration kernel (persistent) ------------------------------------------------------------
 struct GnArgs {
     const BFEntryJ* corr;
     unsigned N, C;
@@ -354,12 +355,48 @@ __device__ __forceinline__ float grid_sum_after_sync(const float* partials, unsi
     return tot;
 }
 
-// kCluster = false: cooperative launch, cg grid barrier (any N).  kCluster = true: ONE thread-block cluster of <= 16 CTAs x 1024
-// threads, hardware cluster barrier (~0.4 us instead of ~3 us) -- the PCG of a <= few-thousand-image problem is barrier-bound.
-template <bool kCluster>
-struct GridBarrier {
-    __device__ __forceinline__ void sync() const {
-        if (kCluster) { __threadfence(); cg::this_cluster().sync(); } else cg::this_grid().sync();
+// How gn_iteration_kernel's G CTAs of BF_SOLVER_THREADS threads run.  Every order-sensitive float sum of the kernel depends only on
+// that partition: a thread's serial sum, the warp tree, a CTA's warp sums added in order (block_sum), the G CTA partials combined by
+// grid_sum_after_sync.
+//  * CoopGrid: G real CTAs, cooperative launch, grid barriers (any N).
+//  * OneCtaGrid: ONE CTA of G x BF_SOLVER_THREADS threads (G <= 4).  Thread t is the cooperative grid's thread t, so rows map to
+//    threads and warps as there; barriers are __syncthreads, and sum() forms the G partials and their total in exactly the shape
+//    above -- bit-identical results.  At the local solve's size the PCG iteration is barrier- and L2-latency-bound.
+struct CoopGrid {
+    static constexpr int kThreads = BF_SOLVER_THREADS;
+    static constexpr bool kPeers = true;
+    __device__ __forceinline__ void sync() const { cg::this_grid().sync(); }
+    // grid-wide sum of every thread's v, the same bits in every thread; partials: [gridDim.x] scratch
+    __device__ __forceinline__ float sum(float v, float* partials, float* sRed) const {
+        v = block_sum(v, sRed);
+        if (threadIdx.x == 0) partials[blockIdx.x] = v;
+        sync();
+        return grid_sum_after_sync(partials, gridDim.x, sRed);
+    }
+};
+struct OneCtaGrid {
+    static constexpr int kThreads = 4 * BF_SOLVER_THREADS;
+    static constexpr bool kPeers = false;
+    __device__ __forceinline__ void sync() const { __syncthreads(); }
+    __device__ __forceinline__ float sum(float v, float*, float* sRed) const {
+        v = warp_sum(v);
+        if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5] = v;
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            const unsigned G = blockDim.x / BF_SOLVER_THREADS, b = threadIdx.x;
+            float g = 0.0f;                                      // grid_sum_after_sync: lane b adds partial b (G <= 32)
+            if (b < G) {
+                float tot = 0.0f;                                // block_sum of virtual CTA b
+                for (unsigned w = 0; w < BF_SOLVER_THREADS / 32; ++w) tot += sRed[b * (BF_SOLVER_THREADS / 32) + w];
+                g += tot;
+            }
+            g = warp_sum(g);
+            if (b == 0) sRed[0] = g;
+        }
+        __syncthreads();
+        const float tot = sRed[0];
+        __syncthreads();
+        return tot;
     }
 };
 
@@ -384,10 +421,10 @@ __device__ __forceinline__ void peer_barrier(const GnArgs& a, unsigned seq, Grid
     __syncthreads();
 }
 
-template <bool kCluster, int kThreads>
-__global__ void __launch_bounds__(kThreads)
+template <class Grid>
+__global__ void __launch_bounds__(Grid::kThreads)
 gn_iteration_kernel(const GnArgs a) {
-    GridBarrier<kCluster> grid;
+    Grid grid;
     __shared__ float sRed[32];
     if (__ldcg(&a.scal[SC_DONE]) != 0) return;                 // an earlier GN iteration converged (uniform for the grid)
     const unsigned tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
@@ -500,12 +537,9 @@ gn_iteration_kernel(const GnArgs a) {
         st3(a.pRot, v, p0r); st3(a.pTrans, v, p0t);
         part += dot(resRot, p0r) + dot(resTrans, p0t);
     }
-    part = block_sum(part, sRed);
-    if (threadIdx.x == 0) a.partials[a.maxGrid + blockIdx.x] = part;      // second array: the first is rewritten by PCG step A
-    grid.sync();
-    float rDotzOld = grid_sum_after_sync(a.partials + a.maxGrid, gridDim.x, sRed);
+    float rDotzOld = grid.sum(part, a.partials + a.maxGrid, sRed);        // second array: the first is rewritten by PCG step A
 
-    const bool peerMode = !kCluster && a.world > 1;
+    const bool peerMode = Grid::kPeers && a.world > 1;
     // (3) PCG iterations (SolverBundling.cu:1024-1108): rows are dealt to warps; lanes split a row's segments
     const unsigned warpsPerBlock = blockDim.x / 32, gwarp = blockIdx.x * warpsPerBlock + (threadIdx.x >> 5), nwarps = gridDim.x * warpsPerBlock;
     const unsigned lane = threadIdx.x & 31;
@@ -578,13 +612,11 @@ gn_iteration_kernel(const GnArgs a) {
                 pAp += pr.x * y[0] + pr.y * y[1] + pr.z * y[2] + pt.x * y[3] + pt.y * y[4] + pt.z * y[5];
             }
         }
-        pAp = block_sum(pAp, sRed);
         float dotProduct;
         if (!peerMode) {
-            if (threadIdx.x == 0) a.partials[blockIdx.x] = pAp;
-            grid.sync();
-            dotProduct = grid_sum_after_sync(a.partials, gridDim.x, sRed);
+            dotProduct = grid.sum(pAp, a.partials, sRed);
         } else {
+            pAp = block_sum(pAp, sRed);
             if (threadIdx.x < (unsigned)a.world) peer_partials(a.peer[threadIdx.x], a.peerMaxN, a.maxGrid, par)[(size_t)a.rank * a.maxGrid + blockIdx.x] = pAp;   // pAp is uniform in the CTA
             peer_barrier(a, a.seqBase + lin + 1u, grid);
             // every rank adds the same world x grid partial sums in the same order: identical bits everywhere
@@ -621,10 +653,7 @@ gn_iteration_kernel(const GnArgs a) {
             st3(a.zRot, v, zR); st3(a.zTrans, v, zT);
             zr += dot(zR, rR) + dot(zT, rT);
         }
-        zr = block_sum(zr, sRed);
-        if (threadIdx.x == 0) a.partials[a.maxGrid + blockIdx.x] = zr;
-        grid.sync();
-        const float rDotzNew = grid_sum_after_sync(a.partials + a.maxGrid, gridDim.x, sRed);
+        const float rDotzNew = grid.sum(zr, a.partials + a.maxGrid, sRed);
         if (fabsf(dotProduct) < 5e-7f) last = true;                     // ENABLE_EARLY_OUT (:1088-1093)
         // C: the new direction's coefficient; the direction itself is formed by the next mat-vec (+ Lie update on the last
         //    iteration, LieDerivUtil.h:301-307)
@@ -1188,43 +1217,11 @@ static int run_gn(const BFSolverInput* in, const BFSolverState* st, const BFSolv
     }
     void* args[] = { (void*)&a };
     ++g_launchCount;
-    // Path 1: one thread-block cluster (hardware barrier).  Chosen when a cluster's warps cover the rows within ~8 rows per warp.
-    static int clusterCap = -1;             // largest launchable cluster size for the 1024-thread variant (0 = unavailable)
-    static int variant = -1;                // BF_SOLVER_BARRIER=cluster selects the cluster variant (measured slower: 20.6 vs 12.8 us per
-                                            // PCG iteration at N = 500 -- the iteration is L2-latency-bound, not barrier-bound, and 16 SMs
-                                            // give it less memory parallelism than 63); default is the cooperative grid
-    if (variant < 0) { const char* e = getenv("BF_SOLVER_BARRIER"); variant = (e && e[0] == 'c') ? 1 : 0; }
-    if (clusterCap < 0) {
-        clusterCap = 0;
-        auto kern = gn_iteration_kernel<true, 1024>;
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
-            for (int cs = 16; cs >= 2; cs >>= 1) {
-                cudaLaunchConfig_t cfg = {};
-                cfg.gridDim = dim3(cs); cfg.blockDim = dim3(1024); cfg.dynamicSmemBytes = 0;
-                cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = cs; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-                cfg.attrs = &at; cfg.numAttrs = 1;
-                int nClusters = 0;
-                if (cudaOccupancyMaxActiveClusters(&nClusters, kern, &cfg) == cudaSuccess && nClusters >= 1) { clusterCap = cs; break; }
-            }
-        }
-        (void)cudaGetLastError();
-    }
-    if (variant == 1 && clusterCap >= 2 && a.N <= (unsigned)clusterCap * 32u * 8u) {
-        int cs = 2;
-        while (cs < clusterCap && (unsigned)cs * 32u < a.N) cs <<= 1;          // one row per warp when possible
-        if (a.N <= 32) cs = 1;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(cs); cfg.blockDim = dim3(1024); cfg.dynamicSmemBytes = 0; cfg.stream = stream();
-        cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = cs; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-        cfg.attrs = &at; cfg.numAttrs = 1;
-        BF_CHECK(cudaLaunchKernelEx(&cfg, gn_iteration_kernel<true, 1024>, a));
-        return 0;
-    }
-    // Path 2: cooperative grid, enough CTAs to give every row a warp, never more than are co-resident
+    // G CTAs: enough to give every row a warp, never more than are co-resident
     static int maxCoResident = 0;
     if (!maxCoResident) {
         int perSm = 0;
-        BF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, gn_iteration_kernel<false, BF_SOLVER_THREADS>, BF_SOLVER_THREADS, 0));
+        BF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, gn_iteration_kernel<CoopGrid>, BF_SOLVER_THREADS, 0));
         maxCoResident = perSm * num_sms();
     }
     int grid = (int)((a.N + (BF_SOLVER_THREADS / 32) - 1) / (BF_SOLVER_THREADS / 32));
@@ -1232,7 +1229,14 @@ static int run_gn(const BFSolverInput* in, const BFSolverState* st, const BFSolv
     if (grid > maxCoResident) grid = maxCoResident;
     if (grid > ws->maxGrid) grid = ws->maxGrid;
     if (grid < 1) grid = 1;
-    BF_CHECK(cudaLaunchCooperativeKernel((void*)gn_iteration_kernel<false, BF_SOLVER_THREADS>, dim3(grid), dim3(BF_SOLVER_THREADS), args, 0, stream()));
+    // Small problems: the G CTAs as one CTA (same bits, no grid barrier).  H100: 5.9 vs 9.3 us per PCG iteration at N = 11, but
+    // 7.8 vs 7.4 at N = 32, where the mat-vec of 32 rows on one SM costs more than the barriers it saves.
+    if (a.world == 1 && a.N <= BF_SOLVER_ONE_CTA_MAX_N && grid * BF_SOLVER_THREADS <= OneCtaGrid::kThreads) {
+        gn_iteration_kernel<OneCtaGrid><<<1, grid * BF_SOLVER_THREADS, 0, stream()>>>(a);
+        BF_CHECK(cudaGetLastError());
+        return 0;
+    }
+    BF_CHECK(cudaLaunchCooperativeKernel((void*)gn_iteration_kernel<CoopGrid>, dim3(grid), dim3(BF_SOLVER_THREADS), args, 0, stream()));
     return 0;
 }
 

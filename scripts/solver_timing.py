@@ -1,4 +1,7 @@
-"""CUDA-event timing of the solver at local / global sizes (development aid)."""
+"""CUDA-event timing of the solver at local / global sizes (development aid).
+
+usage: solver_timing.py [POSE_DIR]  -- with POSE_DIR, the solved poses of every size are also saved there as
+poses_N<N>.npz (rot, trans), so that two builds can be compared bit for bit."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -22,4 +25,7 @@ for (N, deg, gn, pcg) in [(11, 10, 2, 100), (32, 10, 3, 150), (64, 12, 3, 150), 
     b.record(); torch.cuda.synchronize()
     st = sol.getStats()
     ms = a.elapsed_time(b) / 10
+    if len(sys.argv) > 1:
+        os.makedirs(sys.argv[1], exist_ok=True)
+        np.savez(os.path.join(sys.argv[1], f"poses_N{N}.npz"), rot=rot.cpu().numpy(), trans=trans.cpu().numpy())
     print(json.dumps({"N": N, "C": len(prob["corr"]), "ms_per_solve": ms, "gn": st["gn"], "pcg": st["pcg"], "us_per_pcg_iter": ms * 1e3 / max(1, st["pcg"]), "pairs": st["pairs"]}))
