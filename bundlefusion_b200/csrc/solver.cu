@@ -10,8 +10,9 @@
 //    iteration.  Here the correspondences of one image pair are folded ONCE per Gauss-Newton iteration into a
 //    6x6 block (block-sparse J^T J, both (i,j) and (j,i) stored so a row never needs a transpose), and a PCG
 //    iteration is a block-sparse mat-vec over ~144 B per image pair -- ~25x less traffic, L2-resident;
-//  * one persistent kernel (a cooperative grid; one CTA at small N) runs a whole Gauss-Newton iteration: pose -> matrix, block build, row
-//    reduction, PCG init, all PCG iterations (2 grid barriers each), Lie update, convergence test.  The early-outs
+//  * one persistent kernel (a cooperative grid; one CTA at N <= 16; at 17 <= N <= 128 one thread-block cluster with the PCG system
+//    resident in shared memory) runs a whole Gauss-Newton iteration: pose -> matrix, block build, row reduction, PCG init, all PCG iterations
+//    (2 grid barriers each on the grid, none in the cluster), Lie update, convergence test.  The early-outs
 //    (|p.Ap| < 5e-7, max|delta| < 0.005) are evaluated on the device; later GN launches see a "done" flag;
 //  * every floating-point reduction has a fixed shape (per-segment serial sums, fixed warp trees, partials summed
 //    in CTA order), so results are run-to-run deterministic -- the reference's atomics are not.
@@ -358,13 +359,20 @@ __device__ __forceinline__ float grid_sum_after_sync(const float* partials, unsi
 // How gn_iteration_kernel's G CTAs of BF_SOLVER_THREADS threads run.  Every order-sensitive float sum of the kernel depends only on
 // that partition: a thread's serial sum, the warp tree, a CTA's warp sums added in order (block_sum), the G CTA partials combined by
 // grid_sum_after_sync.
-//  * CoopGrid: G real CTAs, cooperative launch, grid barriers (any N).
+//  * CoopGrid: G real CTAs, cooperative launch, grid barriers (any N).  Every PCG operand is read from L2.
 //  * OneCtaGrid: ONE CTA of G x BF_SOLVER_THREADS threads (G <= 4).  Thread t is the cooperative grid's thread t, so rows map to
 //    threads and warps as there; barriers are __syncthreads, and sum() forms the G partials and their total in exactly the shape
 //    above -- bit-identical results.  At the local solve's size the PCG iteration is barrier- and L2-latency-bound.
+//  * ResidentCluster: the same G CTAs as ONE thread-block cluster (G <= the cluster cap, 16 where the device allows it, else 8;
+//    sharded solves excluded).  Steps (0)-(2) and (4) are the grid's with cluster barriers.  The PCG (pcg_resident) first copies
+//    each warp's row -- its segment blocks, dense pair blocks and diagonal blocks -- into the CTA's shared memory, and every CTA
+//    keeps full-length copies of z, p, r, delta, the preconditioner and Ap.  In a PCG iteration
+//    the mat-vec rows store Ap and the p.Ap partials into every CTA's copy (distributed shared memory, st.async), and every CTA
+//    runs the step / residual / z.r phase for all rows itself once its copy is complete.  Every sum keeps the grid's shape, so results are bit-identical.
 struct CoopGrid {
     static constexpr int kThreads = BF_SOLVER_THREADS;
     static constexpr bool kPeers = true;
+    static constexpr bool kResident = false;
     __device__ __forceinline__ void sync() const { cg::this_grid().sync(); }
     // grid-wide sum of every thread's v, the same bits in every thread; partials: [gridDim.x] scratch
     __device__ __forceinline__ float sum(float v, float* partials, float* sRed) const {
@@ -377,6 +385,7 @@ struct CoopGrid {
 struct OneCtaGrid {
     static constexpr int kThreads = 4 * BF_SOLVER_THREADS;
     static constexpr bool kPeers = false;
+    static constexpr bool kResident = false;
     __device__ __forceinline__ void sync() const { __syncthreads(); }
     __device__ __forceinline__ float sum(float v, float*, float* sRed) const {
         v = warp_sum(v);
@@ -399,6 +408,28 @@ struct OneCtaGrid {
         return tot;
     }
 };
+struct ResidentCluster {
+    static constexpr int kThreads = BF_SOLVER_THREADS;
+    static constexpr bool kPeers = false;
+    static constexpr bool kResident = true;
+    __device__ __forceinline__ void sync() const { __threadfence(); cg::this_cluster().sync(); }
+    __device__ __forceinline__ float sum(float v, float* partials, float* sRed) const {
+        v = block_sum(v, sRed);
+        if (threadIdx.x == 0) partials[blockIdx.x] = v;
+        sync();
+        return grid_sum_after_sync(partials, gridDim.x, sRed);
+    }
+};
+#define BF_RESIDENT_MAX_CLUSTER 16
+#define BF_RESIDENT_ROWS (BF_SOLVER_THREADS / 32)      // rows per CTA: warp w of CTA c owns row 1 + 8c + w
+// Dynamic shared memory of pcg_resident, in 4-byte words; S = N slots per row (a row's segments and dense pairs have distinct
+// neighbours in [0, N)).  Blocks first so that they are 16-byte aligned:
+//   off [R][S][36], dense [R][S][36] (when on), diag [R][2][36] (sparse, dense), vec [8][6N] (z, p0, p1, r, delta, prec, Ap[2];
+//   each rot [N][3] then trans [N][3]), part [2][32], nbr [R][S] int, dnb [R][S] int (when on)
+__host__ __device__ inline size_t resident_smem_words(unsigned N, bool dense) {
+    const size_t R = BF_RESIDENT_ROWS, S = N;
+    return R * S * 36 * (dense ? 2 : 1) + R * 72 + (size_t)48 * N + 64 + R * S * (dense ? 2 : 1);
+}
 
 // Barrier over all GPUs of a sharded solve.  Every thread's remote stores are made visible system-wide, the local grid arrives, one CTA publishes this
 // rank's sequence number in every rank's flag array (release), every CTA waits on its OWN region until all ranks have published it (acquire).
@@ -419,6 +450,228 @@ __device__ __forceinline__ void peer_barrier(const GnArgs& a, unsigned seq, Grid
         } while ((int)(v - seq) < 0);
     }
     __syncthreads();
+}
+
+// 6x6 block times 6-vector, the block in shared memory (16-byte aligned): nine 128-bit loads, then blk_mv's arithmetic
+__device__ __forceinline__ void blk_mv_smem(const float* B, V3 pr, V3 pt, float* y) {
+    float b[36];
+#pragma unroll
+    for (int q = 0; q < 9; ++q) { const float4 f = reinterpret_cast<const float4*>(B)[q]; b[4 * q] = f.x; b[4 * q + 1] = f.y; b[4 * q + 2] = f.z; b[4 * q + 3] = f.w; }
+    blk_mv(b, pr, pt, y);
+}
+// dense pair block M (row orientation: M[r*6+c] couples row image coordinate r to the other image's coordinate c, translation
+// first) times p of the other image, the expression of the grid's mat-vec
+__device__ __forceinline__ void dense_mv(const float* M, V3 pr, V3 pt, float* y) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        y[3 + r] += M[r * 6 + 0] * pt.x + M[r * 6 + 1] * pt.y + M[r * 6 + 2] * pt.z + M[r * 6 + 3] * pr.x + M[r * 6 + 4] * pr.y + M[r * 6 + 5] * pr.z;
+        y[r] += M[(3 + r) * 6 + 0] * pt.x + M[(3 + r) * 6 + 1] * pt.y + M[(3 + r) * 6 + 2] * pt.z + M[(3 + r) * 6 + 3] * pr.x + M[(3 + r) * 6 + 4] * pr.y + M[(3 + r) * 6 + 5] * pr.z;
+    }
+}
+
+// Distributed-shared-memory exchange without a cluster barrier: a cluster barrier's release compiles to a GPU-scope memory barrier
+// (MEMBAR.ALL.GPU), which alone costs more than the rest of a small PCG iteration.  Instead every value goes out with st.async,
+// which counts its bytes off the RECEIVING CTA's transaction barrier; a CTA waits on its own barrier until all bytes of an
+// iteration have landed.
+__device__ __forceinline__ unsigned cluster_addr(unsigned a, unsigned rank) {
+    unsigned r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void st_async(unsigned addr, float v, unsigned mbar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" :: "r"(addr), "r"(__float_as_uint(v)), "r"(mbar) : "memory");
+}
+__device__ __forceinline__ void mbar_expect(unsigned mbar, unsigned bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mbar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(unsigned mbar, unsigned parity) {
+    unsigned done = 0;
+    do {
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mbar), "r"(parity) : "memory");
+    } while (!done);
+}
+
+// x(v) <- exp(delta(v)) x(v) (LieDerivUtil.h:301-307), for the resident PCG.  Not inlined: compiled on its own, the float contraction of
+// this branchy code does not depend on the surrounding kernel, and it then rounds exactly as the cooperative grid's inlined copy does;
+// inlined into pcg_resident it rounded differently in the last bit for some rows.
+__device__ __noinline__ void lie_update_row(const GnArgs& a, unsigned v) {
+    float U[16], Cm[16], P[16];
+    pose_to_matrix(ld3(a.deltaRot, v), ld3(a.deltaTrans, v), U);
+    pose_to_matrix(ld3(a.xRot, v), ld3(a.xTrans, v), Cm);
+    mat4_mul(U, Cm, P);
+    V3 nr, nt;
+    matrix_to_pose(P, nr, nt);
+    st3(a.xRot, v, nr); st3(a.xTrans, v, nt);
+}
+// Step (3) of gn_iteration_kernel<ResidentCluster>: all PCG iterations with the system in shared memory (layout: resident_smem_words).
+// Thread and warp roles are the grid's: warp w of CTA c owns row 1 + 8c + w in the mat-vec, and row v of the step phase is thread v
+// -- of CTA 0 in the grid (N <= 128 < 256), of EVERY CTA here, each on its own copies.  The other CTAs' z.r partials are therefore +0
+// in the grid, and each CTA forms the total in the grid's shape locally.  Called after the barrier that ends step (2); returns the
+// number of PCG iterations run.  On exit delta and the Lie update of x are in global memory, written by CTA 0's thread v.
+__device__ unsigned pcg_resident(const GnArgs& a, bool denseOn, float rDotzOld) {
+    extern __shared__ float4 sDyn4[];
+    __shared__ float sRedA[BF_RESIDENT_ROWS], sRedB[BF_RESIDENT_ROWS];
+    __shared__ __align__(8) unsigned long long sMbar[2];                         // transaction barriers of the Ap / partial buffers, by parity
+    cg::cluster_group cluster = cg::this_cluster();
+    const unsigned N = a.N, S = N, R = BF_RESIDENT_ROWS, C = gridDim.x;
+    const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = threadIdx.x;
+    float* const sOff = reinterpret_cast<float*>(sDyn4);
+    float* const sDen = sOff + (size_t)R * S * 36;                              // only when denseOn
+    float* const sDiag = sDen + (denseOn ? (size_t)R * S * 36 : 0);
+    float* const sVec = sDiag + R * 72;
+    float* const sZ = sVec, * const sP0 = sVec + 6 * N, * const sP1 = sVec + 12 * N, * const sR = sVec + 18 * N, * const sDelta = sVec + 24 * N,
+                 * const sPrec = sVec + 30 * N, * const sAp = sVec + 36 * N;        // sAp: [2][6N] by iteration parity
+    float* const sPart = sVec + 48 * N;                                           // [2][32] p.Ap partials by iteration parity
+    int* const sNbr = reinterpret_cast<int*>(sPart + 64);
+    int* const sDnb = sNbr + (size_t)R * S;                                        // only when denseOn
+
+    // ---- residency: this warp's row, the full vectors ----
+    const unsigned v = 1 + blockIdx.x * R + warp;
+    int ns = 0, nd = 0;
+    if (v < N) {
+        // a row's segments have distinct neighbours and its dense pairs distinct other images, all in [0, N): at most S of each
+        const int rs = a.rowStart[v];
+        ns = min(a.segCount[v], (int)S);
+        for (int sI = (int)lane; sI < ns; sI += 32) sNbr[warp * S + sI] = __ldcg(&a.segs[rs + sI].nbr);
+        const float4* gOff = reinterpret_cast<const float4*>(a.offBlk + 36 * (size_t)rs);
+        float4* lOff = reinterpret_cast<float4*>(sOff + 36 * (size_t)warp * S);
+        for (int q = (int)lane; q < ns * 9; q += 32) lOff[q] = __ldcg(&gOff[q]);
+        for (unsigned q = lane; q < 36; q += 32) sDiag[warp * 72 + q] = __ldcg(&a.diagBlk[36 * (size_t)v + q]);
+        if (denseOn) {
+            const int e0 = a.dnbrStart[v];
+            nd = min(a.dnbrStart[v + 1] - e0, (int)S);
+            for (int q = (int)lane; q < nd * 36; q += 32) {
+                const int e = q / 36, rc = q % 36, r = rc / 6, c = rc % 6;
+                const int2 nb = a.dnbr[e0 + e];
+                if (rc == 0) sDnb[warp * S + e] = nb.x;
+                sDen[36 * ((size_t)warp * S + e) + rc] = a.pairOut[(size_t)nb.y * 90 + 42 + ((v < (unsigned)nb.x) ? r * 6 + c : c * 6 + r)];   // v is the pair's hi image: the transposed block
+            }
+            for (unsigned q = lane; q < 36; q += 32) sDiag[warp * 72 + 36 + q] = a.denseDiag[36 * (size_t)v + q];
+        }
+    }
+    for (unsigned i = t; i < 3 * N; i += blockDim.x) {
+        sP0[i] = __ldcg(&a.pRot[i]); sP0[3 * N + i] = __ldcg(&a.pTrans[i]);
+        sR[i] = __ldcg(&a.rRot[i]); sR[3 * N + i] = __ldcg(&a.rTrans[i]);
+        sPrec[i] = __ldcg(&a.precRot[i]); sPrec[3 * N + i] = __ldcg(&a.precTrans[i]);
+        sDelta[i] = 0.0f; sDelta[3 * N + i] = 0.0f;
+    }
+    // per iteration every CTA receives Ap of the N - 1 rows and the C partials; buffer par serves iterations par, par + 2, ...
+    const unsigned bytesPerIter = 24u * (N - 1) + 4u * C;
+    const unsigned mbar0 = smem_u32(&sMbar[0]);
+    if (t == 0) {
+        for (unsigned p = 0; p < 2; ++p) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mbar0 + 8 * p) : "memory");
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_expect(mbar0, bytesPerIter); mbar_expect(mbar0 + 8, bytesPerIter);
+    }
+    cluster.sync();                                                     // every CTA's barriers are armed before the first store
+
+    unsigned pcgRun = 0;
+    float beta = 0.0f;
+    for (unsigned lin = 0; lin < a.nLin; ++lin) {
+        bool last = (lin == a.nLin - 1);
+        ++pcgRun;
+        const bool fly = lin > 0;
+        const unsigned par = lin & 1u;
+        const float* const curP = par ? sP1 : sP0;                                 // p_k of this iteration (formed below when fly)
+        const float* const prvP = par ? sP0 : sP1;                                 // p_{k-1}
+        float* const ap = sAp + par * 6 * N;
+        float* const part = sPart + par * 32;
+        // A: Ap = H p for this warp's row into every CTA's copy, this CTA's partial p.Ap into every CTA's copy
+        float pAp = 0.0f;
+        if (v < N) {
+            float y[6] = { 0, 0, 0, 0, 0, 0 };
+            for (int sI = (int)lane; sI < ns; sI += 32) {
+                const unsigned o = (unsigned)sNbr[warp * S + sI];
+                if (o == 0 || o >= N) continue;                         // variable 0 is fixed: its p is zero by construction
+                const V3 pr = fly ? ld3(sZ, o) + ld3(prvP, o) * beta : ld3(sP0, o);
+                const V3 pt = fly ? ld3(sZ + 3 * N, o) + ld3(prvP + 3 * N, o) * beta : ld3(sP0 + 3 * N, o);
+                blk_mv_smem(&sOff[36 * ((size_t)warp * S + sI)], pr, pt, y);
+            }
+            for (int e = (int)lane; e < nd; e += 32) {                  // nd = 0 without the dense term
+                const unsigned o = (unsigned)sDnb[warp * S + e];
+                if (o == 0) continue;
+                const V3 pr = fly ? ld3(sZ, o) + ld3(prvP, o) * beta : ld3(sP0, o);
+                const V3 pt = fly ? ld3(sZ + 3 * N, o) + ld3(prvP + 3 * N, o) * beta : ld3(sP0 + 3 * N, o);
+                dense_mv(&sDen[36 * ((size_t)warp * S + e)], pr, pt, y);
+            }
+#pragma unroll
+            for (int k = 0; k < 6; ++k) y[k] = warp_sum(y[k]);
+            if (lane == 0) {
+                const V3 pr = fly ? ld3(sZ, v) + ld3(prvP, v) * beta : ld3(sP0, v);
+                const V3 pt = fly ? ld3(sZ + 3 * N, v) + ld3(prvP + 3 * N, v) * beta : ld3(sP0 + 3 * N, v);
+                blk_mv(&sDiag[warp * 72], pr, pt, y);
+                if (denseOn) dense_mv(&sDiag[warp * 72 + 36], pr, pt, y);
+                pAp += pr.x * y[0] + pr.y * y[1] + pr.z * y[2] + pt.x * y[3] + pt.y * y[4] + pt.z * y[5];
+            }
+#pragma unroll
+            for (int k = 0; k < 6; ++k) y[k] = __shfl_sync(0xffffffffu, y[k], 0);      // lane 0's sums (the tree's bits differ by lane)
+            for (unsigned c = lane; c < C; c += 32) {
+                const unsigned dst = cluster_addr(smem_u32(ap), c), mb = cluster_addr(mbar0 + 8 * par, c);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { st_async(dst + 4 * (3 * v + k), y[k], mb); st_async(dst + 4 * (3 * N + 3 * v + k), y[3 + k], mb); }
+            }
+        }
+        pAp = warp_sum(pAp);
+        if (lane == 0) sRedA[warp] = pAp;
+        __syncthreads();
+        if (t < C) {                                                      // block_sum's total, stored into CTA t's partials
+            float tot = 0.0f;
+            for (unsigned w = 0; w < R; ++w) tot += sRedA[w];
+            st_async(cluster_addr(smem_u32(part + blockIdx.x), t), tot, cluster_addr(mbar0 + 8 * par, t));
+        }
+        // every row's Ap and every partial of this iteration have landed here.  A CTA reaches iteration lin + 2 (the next use of this
+        // buffer) only after receiving this CTA's rows of lin + 1, which are sent after this CTA's last read of the buffer below.
+        mbar_wait(mbar0 + 8 * par, (lin >> 1) & 1u);
+        if (t == 0) mbar_expect(mbar0 + 8 * par, bytesPerIter);          // re-arm for lin + 2
+        float dotProduct;
+        {                                                                 // grid_sum_after_sync, in every warp
+            float g = 0.0f;
+            if (lane < C) g += part[lane];
+            g = warp_sum(g);
+            dotProduct = __shfl_sync(0xffffffffu, g, 0);
+        }
+        // B: step, residual, preconditioned residual, z.r -- every row, in every CTA
+        float alpha = 0.0f;
+        if (dotProduct > BF_FLOAT_EPSILON) alpha = rDotzOld / dotProduct;
+        float zr = 0.0f;
+        if (t < N && t != 0) {
+            V3 pkR, pkT;
+            if (fly) {
+                float* const cur = par ? sP1 : sP0;
+                pkR = ld3(sZ, t) + ld3(prvP, t) * beta; pkT = ld3(sZ + 3 * N, t) + ld3(prvP + 3 * N, t) * beta;
+                st3(cur, t, pkR); st3(cur + 3 * N, t, pkT);
+            } else { pkR = ld3(curP, t); pkT = ld3(curP + 3 * N, t); }
+            st3(sDelta, t, ld3(sDelta, t) + pkR * alpha);
+            st3(sDelta + 3 * N, t, ld3(sDelta + 3 * N, t) + pkT * alpha);
+            const V3 rR = ld3(sR, t) - ld3(ap, t) * alpha, rT = ld3(sR + 3 * N, t) - ld3(ap + 3 * N, t) * alpha;
+            st3(sR, t, rR); st3(sR + 3 * N, t, rT);
+            const V3 zR = mulv(ld3(sPrec, t), rR), zT = mulv(ld3(sPrec + 3 * N, t), rT);
+            st3(sZ, t, zR); st3(sZ + 3 * N, t, zT);
+            zr += dot(zR, rR) + dot(zT, rT);
+        }
+        zr = warp_sum(zr);
+        if (lane == 0) sRedB[warp] = zr;
+        __syncthreads();
+        float rDotzNew;
+        {                                                                 // the grid's shape: partial 0 = this CTA's rows, partials 1..C-1 = +0
+            float tot = 0.0f;
+            for (unsigned w = 0; w < R; ++w) tot += sRedB[w];
+            float g = 0.0f;
+            if (lane < C) g += (lane == 0) ? tot : 0.0f;
+            g = warp_sum(g);
+            rDotzNew = __shfl_sync(0xffffffffu, g, 0);
+        }
+        if (fabsf(dotProduct) < 5e-7f) last = true;                     // ENABLE_EARLY_OUT (:1088-1093)
+        beta = 0.0f;
+        if (rDotzOld > BF_FLOAT_EPSILON) beta = rDotzNew / rDotzOld;
+        if (last && blockIdx.x == 0 && t < N && t != 0) {
+            st3(a.deltaRot, t, ld3(sDelta, t)); st3(a.deltaTrans, t, ld3(sDelta + 3 * N, t));
+            lie_update_row(a, t);
+        }
+        rDotzOld = rDotzNew;
+        if (last) break;
+    }
+    return pcgRun;
 }
 
 template <class Grid>
@@ -549,7 +802,8 @@ gn_iteration_kernel(const GnArgs a) {
     // vectors that ARE complete, and each row's owner stores its own p_k(v) into the other of two ping-pong buffers (nobody
     // reads that buffer during this mat-vec).  The expression, and therefore every bit, is the one the stored update had.
     float beta = 0.0f;
-    for (unsigned lin = 0; lin < a.nLin; ++lin) {
+    if constexpr (Grid::kResident) pcgRun = pcg_resident(a, denseOn, rDotzOld);
+    for (unsigned lin = 0; !Grid::kResident && lin < a.nLin; ++lin) {      // the grid's PCG, operands in L2
         bool last = (lin == a.nLin - 1);
         ++pcgRun;
         const bool fly = lin > 0;
@@ -1234,6 +1488,43 @@ static int run_gn(const BFSolverInput* in, const BFSolverState* st, const BFSolv
     if (a.world == 1 && a.N <= BF_SOLVER_ONE_CTA_MAX_N && grid * BF_SOLVER_THREADS <= OneCtaGrid::kThreads) {
         gn_iteration_kernel<OneCtaGrid><<<1, grid * BF_SOLVER_THREADS, 0, stream()>>>(a);
         BF_CHECK(cudaGetLastError());
+        return 0;
+    }
+    // Up to 128 images: the G CTAs as one cluster with the PCG system in shared memory (same bits, no barrier in the PCG loop).
+    // H100 80GB HBM3, 400 W limit, scripts/solver_timing.py, solve time / PCG iterations against the cooperative grid: 2.3 vs 7.3 us
+    // at N = 32, 3.2 vs 8.2 at 64, 3.5 vs 8.4 at 128.  At N = 11 the cluster also beat the one-CTA kernel (4.2 vs 5.4 us) with the
+    // same poses on synthetic problems, but one frame-loop run's outputs differed from the one-CTA build's, and the frame loop's
+    // outputs also vary between runs of one build; until that is settled N <= 16 stays on one CTA.
+    // The cap is the largest launchable cluster, probed once: 16 where the device allows non-portable sizes, else 8.
+    static int clusterCap = 0, maxDynSmem = 0;
+    if (!clusterCap) {
+        auto kern = gn_iteration_kernel<ResidentCluster>;
+        int dev = 0, optin = 0;
+        cudaFuncAttributes fa;
+        BF_CHECK(cudaGetDevice(&dev));
+        BF_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        BF_CHECK(cudaFuncGetAttributes(&fa, kern));
+        maxDynSmem = optin - (int)fa.sharedSizeBytes;
+        BF_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, maxDynSmem));
+        clusterCap = 8;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
+            const unsigned n16 = BF_RESIDENT_MAX_CLUSTER * BF_RESIDENT_ROWS;
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(BF_RESIDENT_MAX_CLUSTER); cfg.blockDim = dim3(BF_SOLVER_THREADS); cfg.dynamicSmemBytes = sizeof(float) * resident_smem_words(n16, false);
+            cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = BF_RESIDENT_MAX_CLUSTER; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+            cfg.attrs = &at; cfg.numAttrs = 1;
+            int nClusters = 0;
+            if (cudaOccupancyMaxActiveClusters(&nClusters, kern, &cfg) == cudaSuccess && nClusters >= 1) clusterCap = BF_RESIDENT_MAX_CLUSTER;
+        }
+        (void)cudaGetLastError();
+    }
+    const size_t smem = sizeof(float) * resident_smem_words(a.N, dense);
+    if (a.world == 1 && grid <= clusterCap && smem <= (size_t)maxDynSmem) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(BF_SOLVER_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream();
+        cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = grid; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+        cfg.attrs = &at; cfg.numAttrs = 1;
+        BF_CHECK(cudaLaunchKernelEx(&cfg, gn_iteration_kernel<ResidentCluster>, a));
         return 0;
     }
     BF_CHECK(cudaLaunchCooperativeKernel((void*)gn_iteration_kernel<CoopGrid>, dim3(grid), dim3(BF_SOLVER_THREADS), args, 0, stream()));
