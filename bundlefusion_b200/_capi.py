@@ -165,6 +165,7 @@ SOLVER_SYMBOLS = [
     "convertLiePosesToMatricesCU", "convertMatricesToPosesCU", "convertPosesToMatricesCU",
     "bfSolverSolve", "bfSolverGetStats", "bfSolverMaxResidual", "bfSolverWorkspaceBytes", "bfSolverReleaseWorkspace", "bfSolverReserveWorkspace",
     "bfSolverDebugDenseSystem", "bfSolverPeerCreate", "bfSolverPeerConnect", "bfSolverPeerDisconnect",
+    "bfSolverSetGridPolicy", "bfSolverGetLaunchInfo",
 ]
 
 
@@ -336,6 +337,9 @@ def lib() -> C.CDLL:
     L.convertPosesToMatricesCU.restype = None
     L.bfSolverSolve.argtypes = [P(BFSolverInput), P(BFSolverState), P(BFSolverParameters)]
     L.bfSolverGetStats.argtypes = [P(BFSolverState), C.c_ulonglong * 8]
+    L.bfSolverSetGridPolicy.argtypes = [C.c_int]
+    L.bfSolverSetGridPolicy.restype = C.c_int
+    L.bfSolverGetLaunchInfo.argtypes = [P(BFSolverState), C.c_int * 4]
     L.bfSolverMaxResidual.argtypes = [P(BFSolverInput), P(BFSolverState), P(BFSolverParameters), vp]
     L.bfSolverWorkspaceBytes.argtypes = [C.c_uint, C.c_uint]
     L.bfSolverWorkspaceBytes.restype = C.c_size_t

@@ -18,6 +18,7 @@
 //    in CTA order), so results are run-to-run deterministic -- the reference's atomics are not.
 #include <cooperative_groups.h>
 
+#include <atomic>
 #include <cstring>
 #include <map>
 #include <mutex>
@@ -65,6 +66,8 @@ __device__ void mat4_inverse(const float* m, float* out) {
 // ---- workspace --------------------------------------------------------------------------------------------
 struct Segment { int nbr; int start; int count; int _pad; };      // one (row image, neighbour image) run of a row
 enum { SC_DONE = 0, SC_GN_RUN = 1, SC_PCG_RUN = 2, SC_NUM_SEG = 3, SC_NUM_VALID = 4, SC_MAXDELTA_BITS = 5, SC_ERROR = 6, SC_DENSE_ON = 7, SC_DENSE_OVERLAP = 8, SC_DENSE_PAIRS = 9, SC_NUM = 16 };
+// values of scal[SC_ERROR] (bfSolverGetStats out[5])
+#define BF_SOLVER_ERR_EXCHANGE_TIMEOUT 2u      // pcg_resident: the bytes of a PCG iteration did not all arrive within BF_MBAR_TIMEOUT_NS
 
 struct SolverWs {
     unsigned maxImages = 0, maxCorr = 0;
@@ -100,6 +103,7 @@ struct SolverWs {
     int rank = 0, world = 1; float* region = nullptr; float* peer[BF_SOLVER_MAX_PEERS] = {}; bool peerOpened[BF_SOLVER_MAX_PEERS] = {}; unsigned peerSeq = 0;
     const void* owner[4] = { nullptr, nullptr, nullptr, nullptr };   // the caller's d_deltaTrans / d_rRot / d_pRot / d_Ap_XRot: a recycled
                                                                      // d_deltaRot address with other neighbours is another solver object
+    int launchInfo[4] = { 0, 0, 0, 0 };                              // last GN launch: policy, G, cluster cap, resident smem limit (bfSolverGetLaunchInfo)
 };
 static void free_ws(SolverWs& w) {
     cudaFree(w.rowCount); cudaFree(w.rowStart); cudaFree(w.cursor); cudaFree(w.entries); cudaFree(w.nbrs); cudaFree(w.segCount); cudaFree(w.segs);
@@ -484,11 +488,34 @@ __device__ __forceinline__ void st_async(unsigned addr, float v, unsigned mbar) 
 __device__ __forceinline__ void mbar_expect(unsigned mbar, unsigned bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mbar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(unsigned mbar, unsigned parity) {
-    unsigned done = 0;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mbar), "r"(parity) : "memory");
-    } while (!done);
+// up to 1024 probes of the phase in one tight PTX loop (written in C++, the loop's exits cost convergence barriers on every probe)
+__device__ __forceinline__ bool mbar_try_wait(unsigned mbar, unsigned parity) {
+    unsigned done;
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .u32 k;\n\tmov.u32 k, 1024;\n"
+                 "BF_MBAR_PROBE_%=:\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+                 "@p bra BF_MBAR_DONE_%=;\n\t"
+                 "sub.u32 k, k, 1;\n\t"
+                 "setp.ne.u32 p, k, 0;\n\t"
+                 "@p bra BF_MBAR_PROBE_%=;\n"
+                 "BF_MBAR_DONE_%=:\n\t"
+                 "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mbar), "r"(parity) : "memory");
+    return done != 0;
+}
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+// A legitimate wait is a few microseconds.  The bound turns a wrong byte count or a missing sender into an error flag instead of a hung device.
+#define BF_MBAR_TIMEOUT_NS 1000000000ull
+// false: the phase did not complete within BF_MBAR_TIMEOUT_NS.  The clock is read once per 1024 probes, off the path of the common short wait.
+__device__ __forceinline__ bool mbar_wait(unsigned mbar, unsigned parity) {
+    if (mbar_try_wait(mbar, parity)) return true;
+    const unsigned long long t0 = globaltimer_ns();
+    while (!mbar_try_wait(mbar, parity))
+        if (globaltimer_ns() - t0 > BF_MBAR_TIMEOUT_NS) return false;
+    return true;
 }
 
 // x(v) <- exp(delta(v)) x(v) (LieDerivUtil.h:301-307), for the resident PCG.  Not inlined: compiled on its own, the float contraction of
@@ -511,6 +538,7 @@ __device__ __noinline__ void lie_update_row(const GnArgs& a, unsigned v) {
 __device__ unsigned pcg_resident(const GnArgs& a, bool denseOn, float rDotzOld) {
     extern __shared__ float4 sDyn4[];
     __shared__ float sRedA[BF_RESIDENT_ROWS], sRedB[BF_RESIDENT_ROWS];
+    __shared__ unsigned sTimedOut;                                                // a thread's wait on sMbar timed out (mbar_wait)
     __shared__ __align__(8) unsigned long long sMbar[2];                         // transaction barriers of the Ap / partial buffers, by parity
     cg::cluster_group cluster = cg::this_cluster();
     const unsigned N = a.N, S = N, R = BF_RESIDENT_ROWS, C = gridDim.x;
@@ -559,6 +587,7 @@ __device__ unsigned pcg_resident(const GnArgs& a, bool denseOn, float rDotzOld) 
     const unsigned bytesPerIter = 24u * (N - 1) + 4u * C;
     const unsigned mbar0 = smem_u32(&sMbar[0]);
     if (t == 0) {
+        sTimedOut = 0u;
         for (unsigned p = 0; p < 2; ++p) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mbar0 + 8 * p) : "memory");
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_expect(mbar0, bytesPerIter); mbar_expect(mbar0 + 8, bytesPerIter);
@@ -621,7 +650,7 @@ __device__ unsigned pcg_resident(const GnArgs& a, bool denseOn, float rDotzOld) 
         }
         // every row's Ap and every partial of this iteration have landed here.  A CTA reaches iteration lin + 2 (the next use of this
         // buffer) only after receiving this CTA's rows of lin + 1, which are sent after this CTA's last read of the buffer below.
-        mbar_wait(mbar0 + 8 * par, (lin >> 1) & 1u);
+        const bool arrived = mbar_wait(mbar0 + 8 * par, (lin >> 1) & 1u);
         if (t == 0) mbar_expect(mbar0 + 8 * par, bytesPerIter);          // re-arm for lin + 2
         float dotProduct;
         {                                                                 // grid_sum_after_sync, in every warp
@@ -651,7 +680,17 @@ __device__ unsigned pcg_resident(const GnArgs& a, bool denseOn, float rDotzOld) 
         }
         zr = warp_sum(zr);
         if (lane == 0) sRedB[warp] = zr;
+        if (!arrived) sTimedOut = 1u;
         __syncthreads();
+        // A timed-out wait leaves the PCG in the whole CTA, before the Lie update.  The other CTAs then time out on this CTA's missing
+        // rows; every CTA passes the cluster barrier of step (4) before it exits, so no store targets an exited CTA's shared memory.
+        // H100 80GB HBM3, 400 W limit, scripts/solver_timing.py against the unbounded wait: +10 / 20 / 30 ns per PCG iteration at
+        // N = 32 / 64 / 128 (2.33 -> 2.34, 3.22 -> 3.24, 3.53 -> 3.56 us).  __syncthreads_or in place of the flag cost ~60 ns, and
+        // this test placed after the beta update ~40 ns.
+        if (sTimedOut) {
+            if (t == 0) a.scal[SC_ERROR] = BF_SOLVER_ERR_EXCHANGE_TIMEOUT;
+            break;
+        }
         float rDotzNew;
         {                                                                 // the grid's shape: partial 0 = this CTA's rows, partials 1..C-1 = +0
             float tot = 0.0f;
@@ -1426,6 +1465,102 @@ static int run_prep(const BFSolverInput* in, const BFSolverState* st, SolverWs* 
     return 0;
 }
 
+// ---- Gauss-Newton launch policy -------------------------------------------------------------------------------------------
+// Which Grid runs gn_iteration_kernel.  Auto picks by size; bfSolverSetGridPolicy forces one process-wide, so that a test can solve one
+// problem under every policy and compare the bits.  A forced policy that cannot run a solve fails it (cudaErrorNotSupported), never falls back.
+enum { BF_POLICY_AUTO = 0, BF_POLICY_GRID = 1, BF_POLICY_ONE_CTA = 2, BF_POLICY_CLUSTER = 3 };
+static std::atomic<int> g_gridPolicy{ BF_POLICY_AUTO };
+
+struct LaunchLimits { int maxCoResident = 0, clusterCap = 0, maxDynSmem = 0; };
+// Probed once per process: the co-resident CTAs of the cooperative grid, the largest launchable cluster of the resident kernel (16 where
+// the device allows non-portable sizes, else 8) and the dynamic shared memory it may use.
+static int launch_limits(LaunchLimits* out) {
+    static std::mutex mu;
+    static LaunchLimits lim;
+    std::lock_guard<std::mutex> lk(mu);
+    if (!lim.clusterCap) {
+        LaunchLimits l;
+        int perSm = 0;
+        BF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, gn_iteration_kernel<CoopGrid>, BF_SOLVER_THREADS, 0));
+        l.maxCoResident = perSm * num_sms();
+        auto kern = gn_iteration_kernel<ResidentCluster>;
+        int dev = 0, optin = 0;
+        cudaFuncAttributes fa;
+        BF_CHECK(cudaGetDevice(&dev));
+        BF_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        BF_CHECK(cudaFuncGetAttributes(&fa, kern));
+        l.maxDynSmem = optin - (int)fa.sharedSizeBytes;
+        BF_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, l.maxDynSmem));
+        l.clusterCap = 8;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
+            const unsigned n16 = BF_RESIDENT_MAX_CLUSTER * BF_RESIDENT_ROWS;
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(BF_RESIDENT_MAX_CLUSTER); cfg.blockDim = dim3(BF_SOLVER_THREADS); cfg.dynamicSmemBytes = sizeof(float) * resident_smem_words(n16, false);
+            cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = BF_RESIDENT_MAX_CLUSTER; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+            cfg.attrs = &at; cfg.numAttrs = 1;
+            int nClusters = 0;
+            if (cudaOccupancyMaxActiveClusters(&nClusters, kern, &cfg) == cudaSuccess && nClusters >= 1) l.clusterCap = BF_RESIDENT_MAX_CLUSTER;
+        }
+        (void)cudaGetLastError();
+        lim = l;
+    }
+    *out = lim;
+    return 0;
+}
+// G CTAs: enough to give every row a warp, never more than are co-resident
+static int gn_grid(unsigned N, const SolverWs* ws, const LaunchLimits& lim) {
+    int grid = (int)((N + (BF_SOLVER_THREADS / 32) - 1) / (BF_SOLVER_THREADS / 32));
+    if (grid > num_sms()) grid = num_sms();
+    if (grid > lim.maxCoResident) grid = lim.maxCoResident;
+    if (grid > ws->maxGrid) grid = ws->maxGrid;
+    if (grid < 1) grid = 1;
+    return grid;
+}
+static bool gn_dense(const BFSolverInput* in, unsigned k) {
+    const float wDepth = in->weightsDenseDepth ? in->weightsDenseDepth[k] : 0.0f, wColor = in->weightsDenseColor ? in->weightsDenseColor[k] : 0.0f;
+    return (wDepth > 0.0f || wColor > 0.0f) && in->d_cacheFrames != nullptr;
+}
+static bool one_cta_can_run(int grid, const SolverWs* ws) { return ws->world == 1 && grid * BF_SOLVER_THREADS <= OneCtaGrid::kThreads; }
+// pcg_resident gives each warp one row (rows 1 .. 8G) and every row's Ap to every CTA: G = ceil(N / 8) CTAs in one cluster
+static bool cluster_can_run(unsigned N, bool dense, int grid, const SolverWs* ws, const LaunchLimits& lim) {
+    return ws->world == 1 && grid <= lim.clusterCap && (unsigned)grid * BF_RESIDENT_ROWS + 1 >= N &&
+           sizeof(float) * resident_smem_words(N, dense) <= (size_t)lim.maxDynSmem;
+}
+static int pick_policy(unsigned N, bool dense, int grid, const SolverWs* ws, const LaunchLimits& lim) {
+    const int forced = g_gridPolicy.load();
+    if (forced != BF_POLICY_AUTO) return forced;          // solve_impl has checked that it can run
+    // Small problems: the G CTAs as one CTA (same bits, no grid barrier).  H100: 5.9 vs 9.3 us per PCG iteration at N = 11, but
+    // 7.8 vs 7.4 at N = 32, where the mat-vec of 32 rows on one SM costs more than the barriers it saves.
+    if (N <= BF_SOLVER_ONE_CTA_MAX_N && one_cta_can_run(grid, ws)) return BF_POLICY_ONE_CTA;
+    // Up to 128 images: the G CTAs as one cluster with the PCG system in shared memory (same bits, no barrier in the PCG loop).
+    // H100 80GB HBM3, 400 W limit, scripts/solver_timing.py, solve time / PCG iterations against the cooperative grid: 2.3 vs 7.3 us
+    // at N = 32, 3.2 vs 8.2 at 64, 3.5 vs 8.4 at 128.  At N = 11 the cluster also beat the one-CTA kernel (4.2 vs 5.4 us).  One bench
+    // frame-loop run once differed between a cluster build and the one-CTA build, but the bench's outputs also vary between runs of one build.
+    // On frame-loop inputs the policies agree bit for bit: tests/test_solver_policies_gpu.py runs a 43-frame stream (local solves at N = 11,
+    // dense term on) under each policy and compares every status field and the trajectory.  Moving N <= 16 to the cluster is a
+    // performance change of its own; until then it stays on one CTA.
+    if (cluster_can_run(N, dense, grid, ws, lim)) return BF_POLICY_CLUSTER;
+    return BF_POLICY_GRID;
+}
+// cudaErrorNotSupported when the forced policy cannot run one of this solve's GN iterations; checked before anything is enqueued
+static int check_forced_policy(const BFSolverInput* in, const BFSolverParameters* par, const SolverWs* ws) {
+    const int forced = g_gridPolicy.load();
+    if (forced == BF_POLICY_AUTO || forced == BF_POLICY_GRID) return 0;
+    LaunchLimits lim;
+    { const int rc = launch_limits(&lim); if (rc) return rc; }
+    const unsigned N = in->numberOfImages;
+    const int grid = gn_grid(N, ws, lim);
+    bool ok = true;
+    if (forced == BF_POLICY_ONE_CTA) ok = one_cta_can_run(grid, ws);
+    else
+        for (unsigned k = 0; k < par->nNonLinearIterations; ++k) ok = ok && cluster_can_run(N, gn_dense(in, k), grid, ws, lim);
+    if (ok) return 0;
+    set_last_error(forced == BF_POLICY_ONE_CTA ? "bfSolverSolve: the forced one-CTA policy needs ceil(N / 8) <= 4 and an unsharded solve"
+                                               : "bfSolverSolve: the forced cluster policy needs ceil(N / 8) <= the cluster cap, the resident system within "
+                                                 "the shared memory limit and an unsharded solve", cudaErrorNotSupported);
+    return (int)cudaErrorNotSupported;
+}
+
 static int run_gn(const BFSolverInput* in, const BFSolverState* st, const BFSolverParameters* par, SolverWs* ws, unsigned nIter, bool isLast) {
     GnArgs a;
     a.corr = in->d_correspondences; a.N = in->numberOfImages; a.C = in->numberOfCorrespondences; a.validImages = in->d_validImages;
@@ -1471,55 +1606,18 @@ static int run_gn(const BFSolverInput* in, const BFSolverState* st, const BFSolv
     }
     void* args[] = { (void*)&a };
     ++g_launchCount;
-    // G CTAs: enough to give every row a warp, never more than are co-resident
-    static int maxCoResident = 0;
-    if (!maxCoResident) {
-        int perSm = 0;
-        BF_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, gn_iteration_kernel<CoopGrid>, BF_SOLVER_THREADS, 0));
-        maxCoResident = perSm * num_sms();
-    }
-    int grid = (int)((a.N + (BF_SOLVER_THREADS / 32) - 1) / (BF_SOLVER_THREADS / 32));
-    if (grid > num_sms()) grid = num_sms();
-    if (grid > maxCoResident) grid = maxCoResident;
-    if (grid > ws->maxGrid) grid = ws->maxGrid;
-    if (grid < 1) grid = 1;
-    // Small problems: the G CTAs as one CTA (same bits, no grid barrier).  H100: 5.9 vs 9.3 us per PCG iteration at N = 11, but
-    // 7.8 vs 7.4 at N = 32, where the mat-vec of 32 rows on one SM costs more than the barriers it saves.
-    if (a.world == 1 && a.N <= BF_SOLVER_ONE_CTA_MAX_N && grid * BF_SOLVER_THREADS <= OneCtaGrid::kThreads) {
+    LaunchLimits lim;
+    { const int rc = launch_limits(&lim); if (rc) return rc; }
+    const int grid = gn_grid(a.N, ws, lim);
+    const int policy = pick_policy(a.N, dense, grid, ws, lim);
+    ws->launchInfo[0] = policy; ws->launchInfo[1] = grid; ws->launchInfo[2] = lim.clusterCap; ws->launchInfo[3] = lim.maxDynSmem;
+    if (policy == BF_POLICY_ONE_CTA) {
         gn_iteration_kernel<OneCtaGrid><<<1, grid * BF_SOLVER_THREADS, 0, stream()>>>(a);
         BF_CHECK(cudaGetLastError());
         return 0;
     }
-    // Up to 128 images: the G CTAs as one cluster with the PCG system in shared memory (same bits, no barrier in the PCG loop).
-    // H100 80GB HBM3, 400 W limit, scripts/solver_timing.py, solve time / PCG iterations against the cooperative grid: 2.3 vs 7.3 us
-    // at N = 32, 3.2 vs 8.2 at 64, 3.5 vs 8.4 at 128.  At N = 11 the cluster also beat the one-CTA kernel (4.2 vs 5.4 us) with the
-    // same poses on synthetic problems, but one frame-loop run's outputs differed from the one-CTA build's, and the frame loop's
-    // outputs also vary between runs of one build; until that is settled N <= 16 stays on one CTA.
-    // The cap is the largest launchable cluster, probed once: 16 where the device allows non-portable sizes, else 8.
-    static int clusterCap = 0, maxDynSmem = 0;
-    if (!clusterCap) {
-        auto kern = gn_iteration_kernel<ResidentCluster>;
-        int dev = 0, optin = 0;
-        cudaFuncAttributes fa;
-        BF_CHECK(cudaGetDevice(&dev));
-        BF_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        BF_CHECK(cudaFuncGetAttributes(&fa, kern));
-        maxDynSmem = optin - (int)fa.sharedSizeBytes;
-        BF_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, maxDynSmem));
-        clusterCap = 8;
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
-            const unsigned n16 = BF_RESIDENT_MAX_CLUSTER * BF_RESIDENT_ROWS;
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(BF_RESIDENT_MAX_CLUSTER); cfg.blockDim = dim3(BF_SOLVER_THREADS); cfg.dynamicSmemBytes = sizeof(float) * resident_smem_words(n16, false);
-            cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = BF_RESIDENT_MAX_CLUSTER; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-            cfg.attrs = &at; cfg.numAttrs = 1;
-            int nClusters = 0;
-            if (cudaOccupancyMaxActiveClusters(&nClusters, kern, &cfg) == cudaSuccess && nClusters >= 1) clusterCap = BF_RESIDENT_MAX_CLUSTER;
-        }
-        (void)cudaGetLastError();
-    }
-    const size_t smem = sizeof(float) * resident_smem_words(a.N, dense);
-    if (a.world == 1 && grid <= clusterCap && smem <= (size_t)maxDynSmem) {
+    if (policy == BF_POLICY_CLUSTER) {
+        const size_t smem = sizeof(float) * resident_smem_words(a.N, dense);
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(grid); cfg.blockDim = dim3(BF_SOLVER_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream();
         cudaLaunchAttribute at; at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = grid; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
@@ -1548,6 +1646,8 @@ static int solve_impl(const BFSolverInput* in, const BFSolverState* st, const BF
     while (cap < in->numberOfCorrespondences) cap <<= 1;
     int rc = get_ws(st, in->maxNumberOfImages > in->numberOfImages ? in->maxNumberOfImages : in->numberOfImages, cap, &ws);
     if (rc) return rc;
+    rc = check_forced_policy(in, par, ws);
+    if (rc) return rc;
     if (rebuild) { rc = run_prep(in, st, ws); if (rc) return rc; }
     else BF_CHECK(cudaMemsetAsync(ws->scal, 0, sizeof(unsigned) * 3, stream()));   // done / counters
     for (unsigned k = 0; k < par->nNonLinearIterations; ++k) {
@@ -1574,6 +1674,20 @@ BF_API int bfSolverGetStats(const BFSolverState* st, unsigned long long out[8]) 
     float md; memcpy(&md, &s[SC_MAXDELTA_BITS], 4);
     out[0] = s[SC_GN_RUN]; out[1] = s[SC_PCG_RUN]; out[2] = s[SC_NUM_SEG] / 2; out[3] = s[SC_DENSE_OVERLAP];
     out[4] = (unsigned long long)(md * 1e6f); out[5] = s[SC_ERROR]; out[6] = s[SC_DONE]; out[7] = s[SC_DENSE_PAIRS];
+    return 0;
+}
+
+BF_API int bfSolverSetGridPolicy(int policy) {
+    if (policy < BF_POLICY_AUTO || policy > BF_POLICY_CLUSTER) return (int)cudaErrorInvalidValue;
+    return g_gridPolicy.exchange(policy);
+}
+
+BF_API int bfSolverGetLaunchInfo(const BFSolverState* st, int out[4]) {
+    if (!st || !out) return (int)cudaErrorInvalidValue;
+    std::lock_guard<std::mutex> lk(g_wsMutex);
+    auto it = g_ws.find(st->d_deltaRot);
+    if (it == g_ws.end()) return (int)cudaErrorInvalidValue;
+    memcpy(out, it->second.launchInfo, sizeof(it->second.launchInfo));
     return 0;
 }
 

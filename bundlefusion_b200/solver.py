@@ -12,6 +12,19 @@ from . import _capi as capi
 from ._capi import BFSolverInput, BFSolverParameters, BFSolverState, BFSolverStateAnalysis
 
 
+# Gauss-Newton grid policies (include/bf_solver.h: bfSolverSetGridPolicy).  Every policy gives the same bits; AUTO picks by problem size.
+GRID_POLICY_AUTO, GRID_POLICY_GRID, GRID_POLICY_ONE_CTA, GRID_POLICY_CLUSTER = 0, 1, 2, 3
+
+
+def set_grid_policy(policy: int) -> int:
+    """Force the Gauss-Newton grid policy of every later solve in this process (GRID_POLICY_AUTO restores the default).  Returns the
+    previous policy.  A forced policy that cannot run a solve makes that solve fail; it never falls back."""
+    rc = capi.lib().bfSolverSetGridPolicy(int(policy))
+    if policy not in (GRID_POLICY_AUTO, GRID_POLICY_GRID, GRID_POLICY_ONE_CTA, GRID_POLICY_CLUSTER):
+        capi.check(rc, "bfSolverSetGridPolicy")
+    return rc
+
+
 class DeviceCache:
     """Device-side array of ``CUDACachedFrame`` structs (FL/CUDACacheUtil.h:41-53) -- what ``CUDACache::getCacheFramesGPU()``
     hands the solver.  Built here from host arrays (dict per frame: depth, campos, intensity, intensityDerivs, normalsU, normals)."""
@@ -185,6 +198,13 @@ class CUDASolverBundling:
         capi.check(self.lib.bfSolverGetStats(C.byref(self.m_solverState), out), "bfSolverGetStats")
         return {"gn": out[0], "pcg": out[1], "pairs": out[2], "max_delta": out[4] * 1e-6, "error": out[5], "converged": out[6],
                 "dense_overlap_pairs": out[3], "dense_weighted_pairs": out[7]}
+
+    def getLaunchInfo(self) -> dict:
+        """The last Gauss-Newton launch of this solver (host-side record, no synchronisation): policy that ran, G (the cooperative grid's
+        CTA count every policy reproduces), the device's cluster cap and the resident kernel's dynamic shared memory limit in bytes."""
+        out = (C.c_int * 4)()
+        capi.check(self.lib.bfSolverGetLaunchInfo(C.byref(self.m_solverState), out), "bfSolverGetLaunchInfo")
+        return {"policy": out[0], "ctas": out[1], "cluster_cap": out[2], "dyn_smem": out[3]}
 
     def getVarToCorrNumEntriesPerRow(self):
         return self.d_numEntriesPerRow

@@ -166,8 +166,21 @@ int bfSolverSolve(const BFSolverInput* input, const BFSolverState* state, const 
 /* statistics of the last bfSolverSolve on this state (synchronises):
  * out[0] = GN iterations run, out[1] = PCG iterations run (all GN iterations), out[2] = image pairs (6x6 blocks),
  * out[3] = overlapping dense image pairs (last GN iteration), out[4] = last max|delta| * 1e6 (fixed point), out[5] = error flag,
- * out[6] = converged early, out[7] = dense pairs with non-zero weight */
+ * out[6] = converged early, out[7] = dense pairs with non-zero weight.  Error flag 2: in the resident cluster's PCG the data of an iteration did
+ * not arrive within a second, and the solve was abandoned (its poses are not meaningful). */
 int bfSolverGetStats(const BFSolverState* state, unsigned long long out[8]);
+
+/* Grid policy of the Gauss-Newton kernel, process-wide: 0 = auto (the default: one CTA at N <= 16, one thread-block cluster with the PCG
+ * system in shared memory for unsharded solves of 17 <= N <= 128 that fit, else the cooperative grid), 1 = cooperative grid, 2 = one CTA,
+ * 3 = resident cluster.  All policies give bit-identical results; forcing one lets a test compare them on one problem.  Returns the previous
+ * policy, or cudaErrorInvalidValue for an unknown one.  A forced policy that cannot run a solve makes bfSolverSolve return
+ * cudaErrorNotSupported before it enqueues anything: one CTA needs ceil(N / 8) <= 4, the cluster needs ceil(N / 8) <= the cluster cap and
+ * the resident system (dense term included where it is on) within the shared memory limit, and neither runs a sharded solve. */
+int bfSolverSetGridPolicy(int policy);
+/* The last Gauss-Newton launch on this state, recorded on the host (does not synchronise): out[0] = policy that ran (1 .. 3 as above),
+ * out[1] = G, the cooperative grid's CTA count that every policy reproduces (the one-CTA policy runs them as G x 256 threads of one CTA),
+ * out[2] = cluster cap probed on this device (8 or 16), out[3] = dynamic shared memory available to the resident cluster kernel, bytes. */
+int bfSolverGetLaunchInfo(const BFSolverState* state, int out[4]);
 
 /* CUDASolverBundling::getMaxResidual's device part (FL/Solver/CUDASolverBundling.cpp:313-329) without the host
  * reduction: writes {max residual, index as float bits} to d_out[0..1].  Asynchronous. */

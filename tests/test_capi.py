@@ -58,6 +58,17 @@ def test_symbol_list_matches_header():
     assert sorted(set(_declared_symbols("bf_marchingcubes.h"))) == sorted(set(capi.MARCHINGCUBES_SYMBOLS))
 
 
+def test_solver_grid_policy_override_is_checked_on_the_host():
+    """bfSolverSetGridPolicy / bfSolverGetLaunchInfo are exported; an unknown policy is refused without a device and leaves the policy as it was"""
+    L = capi.lib()
+    assert hasattr(L, "bfSolverSetGridPolicy") and hasattr(L, "bfSolverGetLaunchInfo")
+    assert L.bfSolverSetGridPolicy(99) == 1                              # cudaErrorInvalidValue
+    assert L.bfSolverSetGridPolicy(-1) == 1
+    assert L.bfSolverSetGridPolicy(3) == 0                               # previous: auto
+    assert L.bfSolverSetGridPolicy(0) == 3
+    assert L.bfSolverGetLaunchInfo(C.byref(capi.BFSolverState()), (C.c_int * 4)()) == 1      # no solve on this state
+
+
 def test_raycast_pod_layouts():
     assert C.sizeof(capi.BFRayCastParams) == 192 and capi.BFRayCastParams.mx.offset == 128 and capi.BFRayCastParams.m_splatMinimum.offset == 160
     assert capi.BFRayCastParams.m_useGradients.offset == 184 and capi.BFRayCastParams.dummy0.offset == 188       # FL/DepthSensing/CUDARayCastParams.h:8-27
