@@ -226,6 +226,10 @@ struct Loop {
     int lastFrameProcessed = -1; bool lastFrameValid = false; int localToSolve = -1; int lastLocalSolved = -1; unsigned numFramesPastEnd = 0;
     unsigned numCompleteTransforms = 0, lastValidCompleteTransform = 0; bool globalTrackingLost = false; int processState = DO_NOTHING; bool useSolve = true;
     unsigned totalNumOptLocalFrames = 0;
+    // end of the recording (bfFrameLoopFinish): K of its first call, the dense end solve of turn K (SBA's global weights switched by
+    // OnlineBundler::processInput, FL/OnlineBundler.cpp:174-189), where it ran and what it covered
+    int finishK = -1; bool finished = false, denseEndSolve = false;
+    int denseTurn = -1; unsigned denseKeyframes = 0, densePairs = 0;
     unsigned numFrames = 0;                      // frames received (CUDAImageManager::getCurrFrameNumber() + 1)
     float currIntegrate[16];
     BFTrajectoryManager* tm = nullptr;
@@ -367,6 +371,9 @@ static int sba_align(Loop& L, Bundler& b, unsigned maxNumIters, unsigned numPCGi
     sv.wS.assign(maxIts, 1.0f); sv.wD.assign(maxIts, 0.0f); sv.wC.assign(maxIts, 0.0f);
     bool useCache = false;
     if (b.isLocal && P.useLocalDense) { for (unsigned i = 0; i < maxIts; ++i) sv.wD[i] = (float)(i + 1); useCache = true; }       // SBA.cpp:28-31
+    if (!b.isLocal && L.denseEndSolve) {                  // Bundler::setSolveWeights at the end of the recording (FL/OnlineBundler.cpp:180-186, SBA.cpp:70-79)
+        sv.wS.assign(3, 1.0f); sv.wD.assign(3, 15.0f); sv.wC.assign(3, 0.0f); useCache = true;
+    }
     const unsigned numImages = sm.numImages;
     FL_OK(sm.pushValid(numImages));                       // valid flags are host-authoritative between stages
     convertMatricesToPosesCU(b.d_trajectory, numImages, sv.d_xRot, sv.d_xTrans, sm.d_valid);
@@ -691,8 +698,14 @@ static int optimize_global(Loop& L) {
             const unsigned countNumFrames = (L.numFramesPastEnd > 0) ? L.numFramesPastEnd : numTotalFrames / P.submapSize;
             const bool removeMax = (countNumFrames % P.numOptPerResidualRemoval) == (P.numOptPerResidualRemoval - 1);
             bool removed = false, valid = false;
-            FL_OK(bundler_optimize(L, g, P.numGlobalNonLinIterations, P.numGlobalLinIterations, false, removeMax, L.numFramesPastEnd > 0, &removed, &valid));
+            const unsigned nNonLin = L.denseEndSolve ? 3u : P.numGlobalNonLinIterations;        // s_numGlobalNonLinIterations = 3 with the end weights (:181)
+            FL_OK(bundler_optimize(L, g, nNonLin, P.numGlobalLinIterations, false, removeMax, L.numFramesPastEnd > 0, &removed, &valid));
             ++L.counters[4];
+            if (L.denseEndSolve) {
+                unsigned long long st[8];
+                FL_OK(bfSolverGetStats(&g.solver.st, st));
+                L.denseTurn = (int)L.numFramesPastEnd - 1; L.denseKeyframes = g.sm.numImages; L.densePairs = (unsigned)st[7];
+            }
             L.status.globalSolved = 1; L.status.globalRemoved = removed ? 1 : 0;
             if (removed)
                 for (unsigned i = 0; i < g.sm.numImages; ++i)
@@ -1002,15 +1015,84 @@ BF_API int bfFrameLoopStepAhead(BFFrameLoop* loop, const float* depth, const uin
     return step_frame(*reinterpret_cast<Loop*>(loop), depth, color, nextDepth, nextColor, onHost, status);
 }
 
+static int past_end_turn(Loop& L, BFFrameLoopStatus* status) {
+    memset(&L.status, 0, sizeof(L.status));
+    L.status.frame = L.numFrames - 1; L.status.localSolved = -1; L.status.lastMatchedFrame = -1;
+    process_input_past_end(L);
+    return step_common(L, false, L.numFrames - 1, status);
+}
+
 BF_API int bfFrameLoopStepPastEnd(BFFrameLoop* loop, BFFrameLoopStatus* status) {
     if (!loop) return (int)cudaErrorInvalidValue;
     Loop& L = *reinterpret_cast<Loop*>(loop);
     if (L.numFrames == 0) return (int)cudaErrorInvalidValue;
     if (L.ahead.valid) { set_last_error("bfFrameLoopStepPastEnd: a frame announced by bfFrameLoopStepAhead is still pending", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
-    memset(&L.status, 0, sizeof(L.status));
-    L.status.frame = L.numFrames - 1; L.status.localSolved = -1; L.status.lastMatchedFrame = -1;
-    process_input_past_end(L);
-    return step_common(L, false, L.numFrames - 1, status);
+    return past_end_turn(L, status);
+}
+
+BF_API int bfFrameLoopFinish(BFFrameLoop* loop, uint32_t numSolveFramesBeforeExit, uint32_t maxTurns, BFFrameLoopFinishInfo* info) {
+    if (!loop) return (int)cudaErrorInvalidValue;
+    Loop& L = *reinterpret_cast<Loop*>(loop);
+    const unsigned K = numSolveFramesBeforeExit;
+    if (L.numFrames == 0) { set_last_error("bfFrameLoopFinish: no frame has been stepped", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    if (L.ahead.valid) { set_last_error("bfFrameLoopFinish: a frame announced by bfFrameLoopStepAhead is still pending", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    if (L.finishK < 0 && L.numFramesPastEnd > K) {
+        set_last_error("bfFrameLoopFinish: more past-end turns than numSolveFramesBeforeExit have run: the dense end solve's turn has passed", cudaErrorInvalidValue);
+        return (int)cudaErrorInvalidValue;
+    }
+    if (L.finishK >= 0 && (unsigned)L.finishK != K) {
+        set_last_error("bfFrameLoopFinish: numSolveFramesBeforeExit differs from the first call's", cudaErrorInvalidValue);
+        return (int)cudaErrorInvalidValue;
+    }
+    L.finishK = (int)K;
+    const unsigned long long solves0 = L.counters[4], reint0 = L.counters[2];
+    unsigned turns = 0;
+    while (!L.finished && turns < maxTurns) {
+        // OnlineBundler::processInput past the end (FL/OnlineBundler.cpp:171-194): the turn's number is m_numFramesPastEnd before its increment
+        const unsigned t = L.numFramesPastEnd;
+        L.denseEndSolve = t == K && L.lastFrameProcessed < 10000;
+        if (t == K + 1) L.useSolve = false;
+        const int rc = past_end_turn(L, nullptr);
+        L.denseEndSolve = false;
+        if (rc) return rc;
+        ++turns;
+        // DepthSensing.cpp:1114-1126: from turn K + 1 on, regenerate the update lists; none left ends the run (StopScanningAndExit)
+        if (t >= K + 1) {
+            bfTrajectoryGenerateUpdateLists(L.tm);
+            if (bfTrajectoryGetNumActiveOperations(L.tm) == 0) L.finished = true;
+        }
+    }
+    FL_OK(join_tsdf(L));
+    if (info) {
+        memset(info, 0, sizeof(*info));
+        info->turns = turns; info->numFramesPastEnd = L.numFramesPastEnd;
+        info->denseTurn = L.denseTurn; info->denseKeyframes = L.denseKeyframes; info->densePairs = L.densePairs;
+        info->globalSolves = (uint32_t)(L.counters[4] - solves0); info->reintegrations = (uint32_t)(L.counters[2] - reint0);
+        // StopScanningAndExit (DepthSensing.cpp:922-932)
+        std::vector<float> all((size_t)L.P.maxNumFrames * 16);
+        const unsigned n = bfTrajectoryGetOptimizedTransforms(L.tm, all.data());
+        unsigned nValid = 0;
+        for (unsigned f = 0; f < n; ++f) if (all[16 * (size_t)f] != kNegInf) ++nValid;          // PoseHelper::countNumValidTransforms
+        unsigned heapFree = 0;
+        FL_OK(bfTsdfGetHeapFreeCount(&L.hd, &heapFree));
+        info->numTransforms = n; info->numValidTransforms = nValid; info->heapFreeCount = heapFree;
+        info->valid = (heapFree >= 800 && nValid >= (unsigned)std::round(0.5f * (float)n)) ? 1 : 0;
+        info->done = L.finished ? 1 : 0;
+    }
+    return L.finished ? 0 : (int)cudaErrorNotReady;
+}
+
+BF_API int bfFrameLoopGetGlobalProblem(const BFFrameLoop* loop, BFFrameLoopGlobalProblem* out) {
+    if (!loop || !out) return (int)cudaErrorInvalidValue;
+    const Loop& L = *reinterpret_cast<const Loop*>(loop);
+    const Bundler& g = L.global;
+    memset(out, 0, sizeof(*out));
+    out->d_correspondences = g.sm.d_glob; out->numCorrespondences = (uint32_t)g.sm.globNum;
+    out->numKeyframes = g.sm.numImages; out->d_validImages = g.sm.d_valid; out->d_trajectory = g.d_trajectory;
+    out->d_cacheFrames = g.cache.d_frames; out->cacheWidth = g.cache.w; out->cacheHeight = g.cache.h;
+    out->intrinsics[0] = g.cache.K[0]; out->intrinsics[1] = g.cache.K[5]; out->intrinsics[2] = g.cache.K[2]; out->intrinsics[3] = g.cache.K[6];
+    out->maxNumImages = g.solver.maxImages; out->maxCorrPerImage = g.solver.maxCorrPerImage;
+    return 0;
 }
 
 BF_API unsigned int bfFrameLoopGetTrajectory(BFFrameLoop* loop, float* h_out, unsigned int maxFrames) {

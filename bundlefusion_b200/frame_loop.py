@@ -47,6 +47,26 @@ class BFFrameLoopStatus(C.Structure):
         return d
 
 
+class BFFrameLoopFinishInfo(C.Structure):
+    _fields_ = [("turns", C.c_uint32), ("numFramesPastEnd", C.c_uint32), ("denseTurn", C.c_int32), ("denseKeyframes", C.c_uint32), ("densePairs", C.c_uint32),
+                ("globalSolves", C.c_uint32), ("reintegrations", C.c_uint32), ("numTransforms", C.c_uint32), ("numValidTransforms", C.c_uint32),
+                ("heapFreeCount", C.c_uint32), ("valid", C.c_int32), ("done", C.c_int32)]
+
+    def as_dict(self):
+        return {"turns": self.turns, "frames_past_end": self.numFramesPastEnd, "dense_turn": self.denseTurn, "dense_keyframes": self.denseKeyframes,
+                "dense_pairs": self.densePairs, "global_solves": self.globalSolves, "reintegrations": self.reintegrations, "transforms": self.numTransforms,
+                "valid_transforms": self.numValidTransforms, "heap_free": self.heapFreeCount, "valid": bool(self.valid), "done": bool(self.done)}
+
+
+class BFFrameLoopGlobalProblem(C.Structure):
+    _fields_ = [("d_correspondences", C.c_void_p), ("numCorrespondences", C.c_uint32), ("numKeyframes", C.c_uint32), ("d_validImages", C.c_void_p),
+                ("d_trajectory", C.c_void_p), ("d_cacheFrames", C.c_void_p), ("cacheWidth", C.c_uint32), ("cacheHeight", C.c_uint32),
+                ("intrinsics", C.c_float * 4), ("maxNumImages", C.c_uint32), ("maxCorrPerImage", C.c_uint32)]
+
+
+CUDA_ERROR_NOT_READY = 600
+
+
 def default_params(width: int, height: int) -> BFFrameLoopParams:
     L = _bind(capi.lib())
     p = BFFrameLoopParams()
@@ -66,6 +86,8 @@ def _bind(L):
     L.bfFrameLoopStep.argtypes = [vp, vp, vp, C.c_int, C.POINTER(BFFrameLoopStatus)]
     L.bfFrameLoopStepAhead.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.POINTER(BFFrameLoopStatus)]
     L.bfFrameLoopStepPastEnd.argtypes = [vp, C.POINTER(BFFrameLoopStatus)]
+    L.bfFrameLoopFinish.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(BFFrameLoopFinishInfo)]
+    L.bfFrameLoopGetGlobalProblem.argtypes = [vp, C.POINTER(BFFrameLoopGlobalProblem)]
     L.bfFrameLoopGetTrajectory.argtypes = [vp, vp, C.c_uint]
     L.bfFrameLoopGetTrajectory.restype = C.c_uint
     L.bfFrameLoopGetHashData.argtypes = [vp]
@@ -125,6 +147,27 @@ class FrameLoop:
         st = BFFrameLoopStatus()
         capi.check(self.lib.bfFrameLoopStepPastEnd(self._h, C.byref(st)), "bfFrameLoopStepPastEnd")
         return st
+
+    def finish(self, solve_frames_before_exit: int = 30, max_turns: int | None = None) -> dict:
+        """The end of the recording as the reference runs it (bfFrameLoopFinish): sparse global solves up to past-end turn K =
+        solve_frames_before_exit (30 in the reference's shipped settings), the dense global solve at turn K, then re-integration only until every
+        frame is fused at its final pose.  max_turns defaults to K + 2 + ceil(frames / maxFrameFixes): once solving stops no pose changes and each
+        frame needs at most one operation.  Returns the call's info; "done" is False when max_turns ran out first (call again to continue)."""
+        self._bind_stream()
+        if max_turns is None:
+            fixes = max(1, int(self.params.maxFrameFixes))
+            max_turns = int(solve_frames_before_exit) + 2 + (self.counters()["frames"] + fixes - 1) // fixes
+        info = BFFrameLoopFinishInfo()
+        rc = self.lib.bfFrameLoopFinish(self._h, int(solve_frames_before_exit), int(max_turns), C.byref(info))
+        if rc != CUDA_ERROR_NOT_READY:
+            capi.check(rc, "bfFrameLoopFinish")
+        return info.as_dict()
+
+    def global_problem(self) -> BFFrameLoopGlobalProblem:
+        """the keyframe bundle-adjustment problem as the loop holds it (its device pointers, valid until the next loop call)"""
+        out = BFFrameLoopGlobalProblem()
+        capi.check(self.lib.bfFrameLoopGetGlobalProblem(self._h, C.byref(out)), "bfFrameLoopGetGlobalProblem")
+        return out
 
     def trajectory(self, n: int) -> np.ndarray:
         out = np.zeros((n, 4, 4), np.float32)

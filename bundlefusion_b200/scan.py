@@ -3,7 +3,7 @@
 trajectory; FL/FriedLiver.cpp, FL/DepthSensing/DepthSensing.cpp:966-1129, 1180-1230) over this library's pieces: ``sens.SensorDataReader`` -> ``FrameLoop.step`` (look-ahead on
 the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every stage is the C-ABI's.
 
-    python -m bundlefusion_b200.scan scan.sens out.ply [--frames N] [--device cuda:0]
+    python -m bundlefusion_b200.scan scan.sens out.ply [--frames N] [--device cuda:0] [--solve-frames-before-exit 30]
 """
 from __future__ import annotations
 
@@ -28,8 +28,11 @@ class _LoopScene:
 
 
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
-                sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None) -> dict:
-    """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}"""
+                sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None) -> dict:
+    """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
+    solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
+    global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
+    None runs a fixed submapSize + 2 past-end turns."""
     r = SensorDataReader(sens_path)
     hd = r.header
     n = len(r) if max_frames is None else min(len(r), max_frames)
@@ -54,12 +57,18 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
         status.append(st.as_dict())
         cur = nxt
     # after the last frame the reference keeps turning its loop without input (FL/OnlineBundler.cpp:170-197) until the last, partial chunk is solved and the
-    # re-integration list is empty: one chunk's worth of turns plus the frames one solve may move
-    for _ in range(int(P.submapSize) + 2):
-        loop.step_past_end()
+    # re-integration list is empty
+    finish = None
+    if solve_frames_before_exit is not None:
+        finish = loop.finish(solve_frames_before_exit)
+    else:                                                                              # one chunk's worth of turns plus the frames one solve may move
+        for _ in range(int(P.submapSize) + 2):
+            loop.step_past_end()
     loop.join()
     out = {"frames": n, "valid": int(sum(s["validTransform"] for s in status)), "keyframes": loop.counters()["keyframes"], "trajectory": loop.trajectory(n), "status": status,
            "mesh_path": None, "triangles": 0}
+    if finish is not None:
+        out["finish"] = finish
     if ply_path is not None:
         mp = marching_cubes_params(int(P.hash.m_hashNumBuckets), float(P.hash.m_virtualVoxelSize), max_num_triangles)
         mc = CUDAMarchingCubesHashSDF(mp, device)
@@ -103,11 +112,16 @@ def main(argv=None) -> int:
     ap.add_argument("--frames", type=int, default=None); ap.add_argument("--device", default="cuda:0")
     ap.add_argument("--hash-buckets", type=int, default=None); ap.add_argument("--sdf-blocks", type=int, default=None)
     ap.add_argument("--trajectory", default=None, help="write the camera-to-world poses here (one 4x4 per frame, text)")
+    ap.add_argument("--solve-frames-before-exit", type=int, default=None, metavar="K",
+                    help="end the recording as the reference does: global solves for K turns past the last frame, the dense global solve at turn K, then "
+                         "re-integration until every frame is fused at its final pose (the reference's value is 30); without it, a fixed 12 past-end turns")
     a = ap.parse_args(argv)
-    o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks)
+    o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
     summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path")}
+    if "finish" in o:
+        summary["finish"] = o["finish"]                     # its "valid": StopScanningAndExit's verdict on the reconstruction
     gt = recorded_poses(a.sens, a.frames)
     if np.isfinite(gt).all(axis=(1, 2)).sum() >= 3:
         summary["ate"] = ate(o["trajectory"], gt[:len(o["trajectory"])])

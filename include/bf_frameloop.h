@@ -19,8 +19,11 @@
  * The host looks at the device three times per frame (key-point count after detection; match verdict + correspondence count; and, on chunk
  * boundaries, the solve verdicts) -- the reference does so dozens of times (every filter stage copies counts back).
  *
+ * The end of a recording (the dense global solve of USE_GLOBAL_DENSE_AT_END, the solve stop, the re-integration drain and the validity
+ * verdict of StopScanningAndExit) is bfFrameLoopFinish; the mesh is extracted by bf_marchingcubes.h.
+ *
  * What is NOT here: sensors / .sens decoding, rendering (ray cast, D3D11), the multi-threaded hand-over between the reconstruction and
- * bundling threads (the call runs the reference's single-threaded order), end-of-sequence extras (USE_GLOBAL_DENSE_AT_END, marching cubes).
+ * bundling threads (the call runs the reference's single-threaded order), writing the optimised poses back into the recording.
  * Threading: one BFFrameLoop per process / device, calls from one thread (the stages share the library's stream and workspaces).
  */
 #ifndef BF_FRAMELOOP_H
@@ -29,6 +32,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "bf_solver.h"
 #include "bf_tsdf.h"
 
 #ifdef __cplusplus
@@ -116,6 +120,50 @@ int bfFrameLoopStepAhead(BFFrameLoop* loop, const float* depth, const uint8_t* c
 /* After the last frame: the reference keeps calling processInput / process with no new frame (FL/OnlineBundler.cpp:170-197) so that the last,
  * partial chunk is solved and re-integration drains.  One such turn per call. */
 int bfFrameLoopStepPastEnd(BFFrameLoop* loop, BFFrameLoopStatus* status);
+
+typedef struct BFFrameLoopFinishInfo {
+    uint32_t turns;                  /* past-end turns run by this call */
+    uint32_t numFramesPastEnd;       /* past-end turns run in total (bfFrameLoopStepPastEnd's included) */
+    int32_t  denseTurn;              /* the past-end turn the dense global solve ran at, -1 if it has not run */
+    uint32_t denseKeyframes;         /* keyframes N of that solve */
+    uint32_t densePairs;             /* its dense image pairs with non-zero weight (bfSolverGetStats out[7]) */
+    uint32_t globalSolves;           /* global solves run by this call */
+    uint32_t reintegrations;         /* re-integration operations run by this call */
+    uint32_t numTransforms;          /* frames of the optimised trajectory */
+    uint32_t numValidTransforms;     /* of them with a valid pose */
+    uint32_t heapFreeCount;          /* free voxel blocks */
+    int32_t  valid;                  /* StopScanningAndExit's verdict: >= 800 free blocks and >= half the transforms valid */
+    int32_t  done;                   /* the exit condition held: no re-integration operation is left */
+} BFFrameLoopFinishInfo;
+
+/* The end of a recording as the reference runs it with s_numSolveFramesBeforeExit = numSolveFramesBeforeExit (K; the shipped value is 30):
+ * past-end turns, each exactly one bfFrameLoopStepPastEnd turn, numbered on from the turns already run, until the exit condition holds or
+ * maxTurns turns have run.  Turns before K solve as bfFrameLoopStepPastEnd does.  Turn K is USE_GLOBAL_DENSE_AT_END (FL/OnlineBundler.cpp:174-189):
+ * its global solve runs 3 Gauss-Newton iterations with weights sparse 1, dense depth 15, dense colour 0 over the keyframes and their cache
+ * (pairwise, the local solve's dense thresholds), unless the last frame index is 10 000 or more.  From turn K + 1 on nothing is solved
+ * (:190-193) and a turn only re-integrates; at the end of each such turn the TrajectoryManager's update lists are regenerated and the run is
+ * done when no operation is left (FL/DepthSensing/DepthSensing.cpp:1114-1126): every frame is then fused at its final pose.
+ * Returns 0 when done (a further call runs nothing), cudaErrorNotReady when maxTurns ran out first (a later call with the same K continues),
+ * cudaErrorInvalidValue without running anything when no frame has been stepped, an announced look-ahead frame is pending, more than K
+ * past-end turns ran before the first call, or K differs from the first call's.  *info (optional) is filled on 0 and cudaErrorNotReady;
+ * the reconstruction stream is joined into the library stream before the call returns. */
+int bfFrameLoopFinish(BFFrameLoop* loop, uint32_t numSolveFramesBeforeExit, uint32_t maxTurns, BFFrameLoopFinishInfo* info);
+
+/* Test accessor: the global (keyframe) bundle-adjustment problem as the loop holds it -- its own device pointers, valid until the next loop call.
+ * The next global solve of the loop runs on exactly these inputs. */
+typedef struct BFFrameLoopGlobalProblem {
+    const BFEntryJ* d_correspondences;           /* keyframe correspondences */
+    uint32_t numCorrespondences;
+    uint32_t numKeyframes;
+    const int32_t* d_validImages;                /* [numKeyframes] */
+    const float* d_trajectory;                   /* [numKeyframes][16], camera-to-world, row-major */
+    const BFCUDACachedFrame* d_cacheFrames;      /* [numKeyframes] keyframe cache frames */
+    uint32_t cacheWidth, cacheHeight;
+    float    intrinsics[4];                      /* cache-resolution fx, fy, mx, my */
+    uint32_t maxNumImages;                       /* the global solver's capacity (maxNumberOfImages) */
+    uint32_t maxCorrPerImage;
+} BFFrameLoopGlobalProblem;
+int bfFrameLoopGetGlobalProblem(const BFFrameLoop* loop, BFFrameLoopGlobalProblem* out);
 
 /* optimised camera-to-world poses of the first n frames (host, [n][16]; invalid frames all -inf); returns the number written */
 unsigned int bfFrameLoopGetTrajectory(BFFrameLoop* loop, float* h_out, unsigned int maxFrames);
