@@ -103,7 +103,7 @@ TSDF_SYMBOLS = [
     "garbageCollectIdentifyCUDA", "garbageCollectFreeCUDA",
     "bfSetStream", "bfGetStream", "bfGetLastErrorString", "bfTsdfAuxBytes", "bfTsdfReset", "bfTsdfIntegrateFrame",
     "bfTsdfGarbageCollect", "bfTsdfGetHeapFreeCount", "bfTsdfGetNumOccupiedBlocks", "bfTsdfGetLastFrameStats",
-    "bfTsdfReleaseAux", "bfTsdfReintegrateFrame", "bfGetLaunchCount", "bfTsdfSetProfiling", "bfTsdfGetProfile", "bfTsdfGetProfileEx", "bfTsdfSetBlockCull", "bfTsdfSetLanes", "bfTsdfSetArithmetic", "bfTsdfReintegrateBatch", "bfTsdfSetBatching", "bfTsdfSetBatchCull",
+    "bfTsdfReleaseAux", "bfTsdfReintegrateFrame", "bfGetLaunchCount", "bfTsdfSetProfiling", "bfTsdfGetProfile", "bfTsdfGetProfileEx", "bfTsdfSetLanes", "bfTsdfSetArithmetic", "bfTsdfReintegrateBatch", "bfTsdfSetBatching",
 ]
 
 HOST_SYMBOLS = ["bfMat4Inverse", "bfTsdfRunOps"]
@@ -295,13 +295,9 @@ def lib() -> C.CDLL:
     L.bfTsdfAuxBytes.restype = C.c_size_t
     L.bfTsdfReset.argtypes = [P(BFHashDataStruct), P(BFHashParams)]
     L.bfTsdfSetBatching.argtypes = [C.c_int]
-    L.bfTsdfSetBatchCull.argtypes = [C.c_int]
-    L.bfTsdfSetBatchCull.restype = C.c_int
     L.bfTsdfSetBatching.restype = C.c_int
     L.bfTsdfSetArithmetic.argtypes = [C.c_int]
     L.bfTsdfSetArithmetic.restype = C.c_int
-    L.bfTsdfSetBlockCull.argtypes = [C.c_int]
-    L.bfTsdfSetBlockCull.restype = C.c_int
     L.bfTsdfSetLanes.argtypes = [C.c_int]
     L.bfTsdfSetLanes.restype = C.c_int
     L.bfTsdfIntegrateFrame.argtypes = [P(BFHashDataStruct), P(BFHashParams), P(BFDepthCameraData), P(BFDepthCameraParams), C.c_int]

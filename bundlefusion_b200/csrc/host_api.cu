@@ -30,9 +30,7 @@ BF_API int bfTsdfRunOps(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCam
 
 static int run_ops(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraParams* cam, const BFTsdfOp* ops, int numOps,
                    const float* const* d_depthFrames, const uint8_t* const* d_colorFrames) {
-    static int fuse = -1;        // BF_TSDF_FUSE_REINT=0 replays every op separately (A/B measurements)
-    if (fuse < 0) { const char* e = getenv("BF_TSDF_FUSE_REINT"); fuse = (e && e[0] == '0') ? 0 : 1; }
-    const bool batch = fuse && d_colorFrames != nullptr && bf::tsdf_batching_usable() != 0;
+    const bool batch = d_colorFrames != nullptr && bf::tsdf_batching_usable() != 0;
     for (int i = 0; i < numOps; ++i) {
         const BFTsdfOp& op = ops[i];
         if (batch) {
@@ -52,7 +50,7 @@ static int run_ops(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraPa
                 continue;
             }
         }
-        if (fuse && op.kind == BF_TSDF_OP_DEINTEGRATE && i + 1 < numOps && ops[i + 1].kind == BF_TSDF_OP_INTEGRATE && ops[i + 1].frame == op.frame) {
+        if (op.kind == BF_TSDF_OP_DEINTEGRATE && i + 1 < numOps && ops[i + 1].kind == BF_TSDF_OP_INTEGRATE && ops[i + 1].frame == op.frame) {
             // the reference's re-integration pair: one fused pass (bfTsdfReintegrateFrame)
             BFHashParams hpOld = *hp;
             for (int k = 0; k < 16; ++k) hpOld.m_rigidTransform.m[k] = op.pose[k];

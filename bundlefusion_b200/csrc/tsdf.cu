@@ -13,8 +13,7 @@
 //    of the whole 4*numBuckets entry table (reference: .cu:324-384), and leaves its count on
 //    the device; the integrate kernel is a persistent grid that reads that count itself;
 //  * the integrate stencil owns 4 consecutive voxels (48 B = three 16-byte vector accesses)
-//    per thread, touches voxel memory only for threads that pass the truncation test, and
-//    can be preceded by a conservative per-block depth-range cull (off by default, measured);
+//    per thread and touches voxel memory only for threads that pass the truncation test;
 //  * garbage collection is a single fused kernel (identify + unlink + heap push + clear).
 //
 // Compiled with -fmad=false so that float results are bit-identical to oracle/tsdf_oracle.c.
@@ -54,9 +53,7 @@ struct TsdfAux {
     unsigned* ctrs = nullptr;        // see CTR_* below
     int* live = nullptr;             // [numSDFBlocks] number of voxels with weight > 0 in the slot's block
     unsigned char* listFlags = nullptr;   // [numSDFBlocks] per compactified entry: bit0 in old frustum, bit1 in new (fused re-integration)
-    int4* work = nullptr;            // [numSDFBlocks] stencil work list {bx,by,bz, slot | pose bits << 28}: list entries that survive the depth-range cull
-    float2* tiles = nullptr;         // [tilesCap] per 16x16-pixel tile {min, max} of the depths the stencil would accept
-    unsigned tilesCap = 0;
+    int4* work = nullptr;            // [numSDFBlocks] stencil work list {bx,by,bz, slot | pose bits << 28}, one item per list entry
     float2* tilesMulti = nullptr;    // [BF_MULTI_MAX_OPS][tilesMultiPer]: depth tiles of the frames of a re-integration batch
     unsigned tilesMultiPer = 0;
     bool liveValid = false;          // false once something outside integrate/de-integrate changed weights
@@ -355,10 +352,10 @@ __global__ void reset_mutex_kernel(int* mutex, unsigned numBuckets) {
 // unchanged.
 #define BF_ALLOC_SET 1024      // slots of the per-CTA set (power of two); overflow falls back to direct handling
 
-// ---- depth tiles + conservative per-block cull ----------------------------------------------------------------------
+// ---- depth tiles + conservative per-block cull of the batch re-integration ------------------------------------------------
 // tiles[ty * tilesX + tx] = {min, max} over the 16x16-pixel tile of the depths the stencil accepts (`depth != -inf &&
-// depth < maxIntegrationDistance`, .cu:441); {+inf, -inf} when the tile holds none.  Written by alloc_kernel (its CTAs are
-// exactly these tiles) or by depth_tiles_kernel when no allocation precedes the stencil (de-integration).
+// depth < maxIntegrationDistance`, .cu:441); {+inf, -inf} when the tile holds none.  Written by alloc_kernel, whose CTAs are
+// exactly these tiles.
 #define BF_TILE 16
 __device__ __forceinline__ void tile_minmax(const BFHashParams& hp, float d, bool inImage, unsigned tid, float2* sRed /*[8]*/) {
     const bool ok = inImage && d != -INFINITY && d < hp.m_maxIntegrationDistance;
@@ -373,22 +370,11 @@ __device__ __forceinline__ float2 tile_minmax_finish(const float2* sRed) {
     for (int w = 1; w < 8; ++w) { r.x = fminf(r.x, sRed[w].x); r.y = fmaxf(r.y, sRed[w].y); }
     return r;
 }
-__global__ void __launch_bounds__(256)
-depth_tiles_kernel(const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp, const float* __restrict__ depth, float2* tiles) {
-    __shared__ float2 sRed[8];
-    const unsigned tid = threadIdx.y * blockDim.x + threadIdx.x;
-    const unsigned x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    const bool in = x < cp.m_imageWidth && y < cp.m_imageHeight;
-    tile_minmax(hp, in ? __ldg(&depth[y * cp.m_imageWidth + x]) : 0.0f, in, tid, sRed);
-    __syncthreads();
-    if (tid == 0) tiles[blockIdx.y * gridDim.x + blockIdx.x] = tile_minmax_finish(sRed);
-}
 
-// Can ANY voxel of block b pass the stencil's test `on screen && depth valid && |depth - z| < truncation(depth)` for the pose in
-// hp?  Conservative (never false when a voxel passes): the cube of voxel centres is bounded by a camera-space AABB, its
+// Can ANY voxel of block b pass the stencil's test `on screen && depth valid && |depth - z| < truncation(depth)` for the pose
+// Minv?  Conservative (never false when a voxel passes): the cube of voxel centres is bounded by a camera-space AABB, its
 // projection by a pixel rectangle with a pixel of slack, the depths under it by the tile min/max, all with a 1 mm (+ relative)
-// margin that dwarfs the fp32 rounding of the per-voxel projection.  Results are therefore unchanged; ~35 % of the in-frustum
-// blocks of a scan (looking past / short of the surface, or at invalid depth) never reach the stencil.
+// margin that dwarfs the fp32 rounding of the per-voxel projection.  Results are therefore unchanged.
 __device__ __forceinline__ bool block_can_pass_m(float s, float T, float vs, const BFFloat4x4& Minv, const BFDepthCameraParams& cp, const float2* __restrict__ tiles, int tilesX, I3 b) {
     if (!(s >= 0.0f && s < 1.0f && T >= 0.0f && cp.fx > 0.0f && cp.fy > 0.0f && vs > 0.0f)) return true;
     const float* M = Minv.m;
@@ -416,9 +402,6 @@ __device__ __forceinline__ bool block_can_pass_m(float s, float T, float vs, con
         for (int tx = tx0; tx <= tx1; ++tx) { const float2 t = __ldg(&tiles[ty * tilesX + tx]); dmin = fminf(dmin, t.x); dmax = fmaxf(dmax, t.y); }
     if (!(dmax >= dmin)) return false;                      // no acceptable depth under the footprint
     return !(zmin >= dmax * (1.0f + s) + T + eps || zmax <= dmin * (1.0f - s) - T - eps);
-}
-__device__ __forceinline__ bool block_can_pass(const BFHashParams& hp, const BFDepthCameraParams& cp, const float2* __restrict__ tiles, int tilesX, I3 b) {
-    return block_can_pass_m(hp.m_truncScale, hp.m_truncation, hp.m_virtualVoxelSize, hp.m_rigidTransformInverse, cp, tiles, tilesX, b);
 }
 __device__ __forceinline__ I3 unpack_block_key(unsigned long long key) {
     const int lim = 1 << 20;
@@ -539,7 +522,7 @@ alloc_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const
     for (unsigned i = tid; i < BF_ALLOC_SET; i += 256) sSet[i] = 0ull;
     const unsigned x = blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (tiles) {           // this CTA is one 16x16 depth tile: leave its min / max for the per-block cull of the stencil
+    if (tiles) {           // this CTA is one 16x16 depth tile: leave its min / max for the batch cull (compactify_multi_kernel)
         const bool in = x < cp.m_imageWidth && y < cp.m_imageHeight;
         tile_minmax(hp, in ? __ldg(&depth[y * cp.m_imageWidth + x]) : 0.0f, in, tid, sRed);
     }
@@ -603,8 +586,7 @@ alloc_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const
 // Warp-aggregated append; counts accumulate in the counter set `set` (zeroed by the preceding launch).
 __global__ void __launch_bounds__(256)
 compactify_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp,
-                  const int4* __restrict__ slotInfo, unsigned* ctrs, int set,
-                  int4* __restrict__ work, const float2* __restrict__ tiles, int tilesX) {
+                  const int4* __restrict__ slotInfo, unsigned* ctrs, int set, int4* __restrict__ work) {
     const unsigned highWater = ctrs[CTR_HIGH_WATER];
     const unsigned tid = blockIdx.x * blockDim.x + threadIdx.x;
     const int countIdx = set + SET_COUNT, workIdx = set + SET_WORK;       // zeroed by the launch before this one
@@ -612,25 +594,22 @@ compactify_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, 
     const unsigned lane = threadIdx.x & 31;
     for (unsigned base = tid - lane; base < highWater; base += stride) {
         const unsigned slot = base + lane;
-        bool keep = false, probe = false;
+        bool keep = false;
         int4 info = make_int4(0, 0, 0, -1);
         if (slot < highWater) {
             info = __ldcg(&slotInfo[slot]);
             if (info.w >= 0) {
                 I3 b = { info.x, info.y, info.z };
                 keep = block_in_frustum(hp, cp, b);
-                probe = keep && (tiles == nullptr || block_can_pass(hp, cp, tiles, tilesX, b));
             }
         }
         const unsigned ballot = __ballot_sync(0xffffffffu, keep);
         if (ballot) {
-            const unsigned ballotW = __ballot_sync(0xffffffffu, probe);
             unsigned warpBase = 0, workBase = 0;
             if (lane == 0) {
                 warpBase = atomicAdd(&ctrs[countIdx], __popc(ballot));
                 if (work) {
-                    if (ballotW) workBase = atomicAdd(&ctrs[workIdx], __popc(ballotW));
-                    if (ballot != ballotW) atomicAdd(&ctrs[set + SET_CULLED], __popc(ballot) - __popc(ballotW));
+                    workBase = atomicAdd(&ctrs[workIdx], __popc(ballot));
                     atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_E_TOT_LO]), (unsigned long long)__popc(ballot));
                 }
             }
@@ -643,7 +622,7 @@ compactify_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, 
                 e.offset = hd.d_hash[info.w].offset;
                 hd.d_hashCompactified[warpBase + __popc(ballot & ((1u << lane) - 1u))] = e;
             }
-            if (work && probe) work[workBase + __popc(ballotW & ((1u << lane) - 1u))] = make_int4(info.x, info.y, info.z, (int)(slot | (1u << 28)));
+            if (work && keep) work[workBase + __popc(ballot & ((1u << lane) - 1u))] = make_int4(info.x, info.y, info.z, (int)(slot | (1u << 28)));
         }
     }
 }
@@ -677,16 +656,14 @@ __global__ void rebuild_aux_kernel(BFHashDataStruct hd, unsigned numEntries, uns
 // ---- the integrate / de-integrate stencil (CUDASceneRepHashSDF.cu:420-521) --------------
 // 128 threads per SDF block, 4 consecutive voxels (48 B) per thread.  Persistent grid: each CTA
 // walks the compactified list with stride gridDim.x; the list length is read from device memory.
-struct VoxelQuad { uint4 a, b, c; };
-#ifndef BF_SPEC_BLOCKS
+struct VoxelQuad { uint4 a, b, c; };   // 4 voxels = 12 words: v0{a.x,a.y,a.z} v1{a.w,b.x,b.y} v2{b.z,b.w,c.x} v3{c.y,c.z,c.w}
 #define BF_SPEC_BLOCKS 24576u
-#endif   // 4 voxels = 12 words: v0{a.x,a.y,a.z} v1{a.w,b.x,b.y} v2{b.z,b.w,c.x} v3{c.y,c.z,c.w}
 
 __device__ __forceinline__ float clamp_color(float v) { return fmaxf(0.0f, fminf(v, 254.5f)); }
 
 // The stencil is bound by the XU pipe (conversions, roundf and MUFU run at 1/8 rate), not by FMA/ALU issue, so the
-// byte <-> float traffic of the colour update and the float -> pixel conversions are done with exact integer/FMA-pipe
-// identities instead of cvt / frnd.  Each is value-identical to the plain expression in its comment for EVERY input.
+// byte <-> float traffic of the colour update is done with exact integer/FMA-pipe identities instead of cvt / frnd.
+// Each is value-identical to the plain expression in its comment for EVERY input.
 // (float)b for b in [0, 255]
 __device__ __forceinline__ float u8_to_float(unsigned b) { return __uint_as_float(0x4B000000u | b) - 8388608.0f; }
 // (unsigned)clamp_color(roundf(r))   [roundf: half away from zero; cvt.rzi of a value in [0, 254.5]]
@@ -698,16 +675,9 @@ __device__ __forceinline__ unsigned round_clamp_u8(float r) {
     return __float_as_uint(v + 8388608.0f) & 0xffu;            // 254.5 + 2^23 rounds to the even 254 = trunc
 }
 // idx = (unsigned)(int)t and the test idx < limit, t = screen coordinate + 0.5   [cvt.rzi.s32.f32: NaN -> 0, (-1, 0) -> 0]
-#ifndef BF_PIXEL_F2I
-#define BF_PIXEL_F2I 1      // 1: one cvt.rzi per coordinate (XU pipe); 0: the ~10-instruction FMA/ALU-pipe identity below
-#endif
-__device__ __forceinline__ bool pixel_index(float t, unsigned limit, float limitF, unsigned& idx) {
-    if (BF_PIXEL_F2I || limit > (1u << 22)) { idx = (unsigned)(int)t; return idx < limit; }
-    if (t <= -1.0f || t >= limitF) return false;               // NaN passes both tests, as the conversion gives 0
-    const float c = fmaxf(t, 0.0f);                            // fmaxf(NaN, 0) = 0
-    const float n = c + 8388608.0f;                            // 2^23 + rne(c)
-    idx = (__float_as_uint(n) & 0x7FFFFFu) - ((n - 8388608.0f) > c ? 1u : 0u);   // floor(c)
-    return true;
+__device__ __forceinline__ bool pixel_index(float t, unsigned limit, unsigned& idx) {
+    idx = (unsigned)(int)t;
+    return idx < limit;
 }
 
 template <bool kDeIntegrate>
@@ -749,8 +719,8 @@ integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, c
                  const int4* __restrict__ work, int set) {
     const unsigned* countPtr = useListCount ? ctrs + set + SET_COUNT : nullptr;
     const unsigned* workCountPtr = ctrs + set + SET_WORK;
-    // `work` (from the library's own compactify): the list entries that survive the depth-range cull, 16 B each; without it
-    // (reference-named stubs, whose list may come from anywhere) the kernel walks d_hashCompactified itself.
+    // `work` (from the library's own compactify): one 16-byte item per list entry; without it (reference-named stubs, whose
+    // list may come from anywhere) the kernel walks d_hashCompactified itself.
     const unsigned listCount = countPtr ? *countPtr : countOverride;
     const unsigned count = work ? *workCountPtr : listCount;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -759,7 +729,6 @@ integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, c
     }
     const unsigned t = threadIdx.x;
     const unsigned W = cp.m_imageWidth, H = cp.m_imageHeight;
-    const float Wf = (float)W, Hf = (float)H;
     // local voxel coordinates of this thread's first voxel: i = 4t -> x = (4t)%8, y = (4t%64)/8, z = 4t/64
     const int lx = (int)((4 * t) & 7), ly = (int)(((4 * t) & 63) >> 3), lz = (int)((4 * t) >> 6);
     unsigned passed = 0;
@@ -799,7 +768,7 @@ integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, c
             const float sx = pf.x * cp.fx / pf.z + cp.mx;
             const float sy = pf.y * cp.fy / pf.z + cp.my;
             unsigned px, py;
-            if (pixel_index(sx + 0.5f, W, Wf, px) && pixel_index(sy + 0.5f, H, Hf, py) && colorImg != nullptr) {
+            if (pixel_index(sx + 0.5f, W, px) && pixel_index(sy + 0.5f, H, py) && colorImg != nullptr) {
                 const float depth = __ldg(&depthImg[py * W + px]);
                 if (depth != -INFINITY && depth < hp.m_maxIntegrationDistance) {
                     float sdf = depth - pf.z;
@@ -844,161 +813,6 @@ integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, c
     }
 }
 
-// ---- TMA-staged variant of the same stencil -------------------------------------------------------
-// One producer warp streams whole 6144-byte voxel tiles into a 4-deep shared-memory ring with the bulk
-// async-copy engine (cp.async.bulk, mbarrier completion); four consumer warps (128 threads, 4 voxels
-// each) project / gather depth for block k+1 while tile k is in flight, read their 48 bytes from shared
-// memory, and write only the dirty 16-byte pieces back to HBM.  Latency of the entry -> tile dependency
-// is carried by the copy engine instead of by resident warps.
-#define BF_TMA_STAGES 4
-#define BF_TILE_BYTES (BF_SDF_BLOCK_VOXELS * 12)
-
-struct GatherSet {           // what consumer thread t needs to update its 4 voxels of one block
-    float pz[4];             // camera-space z of the voxel centres
-    float depth[4];          // depth at the projected pixel (or -inf)
-    uchar4 col[4];
-    unsigned onscreen;       // bit k: voxel k projects inside the image
-};
-
-__device__ __forceinline__ void gather_block(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depthImg,
-                                             const uchar4* __restrict__ colorImg, int bx, int by, int bz, int lx, int ly, int lz, GatherSet& g) {
-    const unsigned W = cp.m_imageWidth, H = cp.m_imageHeight;
-    g.onscreen = 0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const I3 pi = { bx * BF_SDF_BLOCK_SIZE + lx + k, by * BF_SDF_BLOCK_SIZE + ly, bz * BF_SDF_BLOCK_SIZE + lz };
-        const F3 pf = xform(hp.m_rigidTransformInverse, voxel_to_world(hp, pi));
-        const float sx = pf.x * cp.fx / pf.z + cp.mx;
-        const float sy = pf.y * cp.fy / pf.z + cp.my;
-        const unsigned px = (unsigned)(int)(sx + 0.5f), py = (unsigned)(int)(sy + 0.5f);
-        g.pz[k] = pf.z;
-        g.depth[k] = -INFINITY;
-        g.col[k] = make_uchar4(0, 0, 0, 0);
-        if (px < W && py < H) {
-            g.onscreen |= 1u << k;
-            g.depth[k] = __ldg(&depthImg[py * W + px]);
-            g.col[k] = __ldg(&colorImg[py * W + px]);
-        }
-    }
-}
-
-template <bool kDeIntegrate>
-__global__ void __launch_bounds__(160)
-integrate_tma_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp,
-                     const float* __restrict__ depthImg, const uchar4* __restrict__ colorImg,
-                     const unsigned* __restrict__ countPtr, unsigned countOverride, unsigned* ctrs, int* __restrict__ live, int set) {
-    __shared__ __align__(128) uint4 sTile[BF_TMA_STAGES][BF_TILE_BYTES / 16];
-    __shared__ __align__(8) unsigned long long sFull[BF_TMA_STAGES], sEmpty[BF_TMA_STAGES];
-    __shared__ unsigned sPassed[4];
-
-    const unsigned count = countPtr ? *countPtr : countOverride;
-    if (blockIdx.x == 0 && threadIdx.x == 0 && countPtr) { hd.d_hashCompactifiedCounter[0] = (int)count; ctrs[CTR_E] = count; }
-    const unsigned t = threadIdx.x;
-    const unsigned nLocal = (count > blockIdx.x) ? (count - blockIdx.x - 1) / gridDim.x + 1 : 0;   // blocks this CTA owns
-    if (nLocal == 0 || colorImg == nullptr) return;        // without colour nothing passes (.cu:441-448)
-
-    if (t == 0) {
-#pragma unroll
-        for (int s = 0; s < BF_TMA_STAGES; ++s) { mbar_init(&sFull[s], 1); mbar_init(&sEmpty[s], 4); }
-        mbar_fence_init();
-    }
-    __syncthreads();
-
-    const BFHashEntry* __restrict__ list = hd.d_hashCompactified;
-    if (t >= 128) {
-        // ---------------- producer warp ----------------
-        const unsigned lane = t - 128;
-        unsigned ptrBatch = 0;
-        for (unsigned k = 0; k < nLocal; ++k) {
-            if ((k & 31) == 0) {                                // prefetch the next 32 block pointers, one per lane
-                const unsigned kk = k + lane;
-                ptrBatch = (kk < nLocal) ? (unsigned)__ldg(&list[blockIdx.x + (size_t)kk * gridDim.x].ptr) : 0u;
-            }
-            const unsigned ptr = __shfl_sync(0xffffffffu, ptrBatch, k & 31);
-            const unsigned s = k % BF_TMA_STAGES, use = k / BF_TMA_STAGES;
-            if (lane == 0) {
-                if (use > 0) mbar_wait(&sEmpty[s], (use - 1) & 1);
-                mbar_arrive_expect_tx(&sFull[s], BF_TILE_BYTES);
-                bulk_g2s(&sTile[s][0], hd.d_SDFBlocks + (size_t)ptr, BF_TILE_BYTES, &sFull[s]);
-            }
-            __syncwarp();
-        }
-        return;
-    }
-
-    // ---------------- consumer warps ----------------
-    const int lx = (int)((4 * t) & 7), ly = (int)(((4 * t) & 63) >> 3), lz = (int)((4 * t) >> 6);
-    unsigned passed = 0;
-    auto loadPos = [&](unsigned k, int& x, int& y, int& z, unsigned& p) {
-        const BFHashEntry* e = &list[blockIdx.x + (size_t)k * gridDim.x];
-        x = __ldg(&e->pos[0]); y = __ldg(&e->pos[1]); z = __ldg(&e->pos[2]); p = (unsigned)__ldg(&e->ptr);
-    };
-    int nx = 0, ny = 0, nz = 0; unsigned nptr = 0;              // entry of block k+1
-    unsigned curPtr;
-    GatherSet cur, nxt;
-    {
-        int x0, y0, z0;
-        loadPos(0, x0, y0, z0, curPtr);
-        if (nLocal > 1) loadPos(1, nx, ny, nz, nptr);
-        gather_block(hp, cp, depthImg, colorImg, x0, y0, z0, lx, ly, lz, cur);
-    }
-    for (unsigned k = 0; k < nLocal; ++k) {
-        // (1) start the gathers of block k+1 and the entry load of block k+2
-        int fx = 0, fy = 0, fz = 0; unsigned fptr = 0;
-        const bool haveNext = (k + 1 < nLocal);
-        if (haveNext) gather_block(hp, cp, depthImg, colorImg, nx, ny, nz, lx, ly, lz, nxt);
-        if (k + 2 < nLocal) loadPos(k + 2, fx, fy, fz, fptr);
-
-        // (2) truncation test of block k (gathers issued one iteration ago)
-        float sdfv[4];
-        unsigned mask = 0;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const float depth = cur.depth[j];
-            sdfv[j] = 0.0f;
-            if (((cur.onscreen >> j) & 1u) && depth != -INFINITY && depth < hp.m_maxIntegrationDistance) {
-                float sdf = depth - cur.pz[j];
-                const float trunc = truncation(hp, depth);
-                if (fabsf(sdf) < trunc) { sdfv[j] = (sdf >= 0.0f) ? fminf(trunc, sdf) : fmaxf(-trunc, sdf); mask |= 1u << j; }
-            }
-        }
-        // (3) tile k: wait for the bulk copy, pull this thread's 48 bytes, release the stage
-        const unsigned s = k % BF_TMA_STAGES;
-        mbar_wait(&sFull[s], (k / BF_TMA_STAGES) & 1);
-        VoxelQuad q;
-        q.a = sTile[s][3 * t]; q.b = sTile[s][3 * t + 1]; q.c = sTile[s][3 * t + 2];
-        __syncwarp();
-        if ((t & 31) == 0) mbar_arrive(&sEmpty[s]);
-        // (4) update + write back dirty 16-byte pieces
-        int liveDelta = 0;
-        if (mask) {
-            uint4* vp = reinterpret_cast<uint4*>(hd.d_SDFBlocks + (size_t)curPtr) + 3 * t;
-            if (mask & 1u) update_voxel<kDeIntegrate>(hp, sdfv[0], cur.col[0], q.a.x, q.a.y, q.a.z, liveDelta);
-            if (mask & 2u) update_voxel<kDeIntegrate>(hp, sdfv[1], cur.col[1], q.a.w, q.b.x, q.b.y, liveDelta);
-            if (mask & 4u) update_voxel<kDeIntegrate>(hp, sdfv[2], cur.col[2], q.b.z, q.b.w, q.c.x, liveDelta);
-            if (mask & 8u) update_voxel<kDeIntegrate>(hp, sdfv[3], cur.col[3], q.c.y, q.c.z, q.c.w, liveDelta);
-            if (mask & 0x3u) vp[0] = q.a;
-            if (mask & 0x6u) vp[1] = q.b;
-            if (mask & 0xCu) vp[2] = q.c;
-            passed += __popc(mask);
-        }
-        if (__any_sync(0xffffffffu, liveDelta != 0)) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) liveDelta += __shfl_xor_sync(0xffffffffu, liveDelta, o);
-            if ((t & 31) == 0 && liveDelta != 0) atomicAdd(&live[curPtr / BF_SDF_BLOCK_VOXELS], liveDelta);
-        }
-        cur = nxt; curPtr = nptr;
-        nx = fx; ny = fy; nz = fz; nptr = fptr;
-    }
-    passed = warp_sum_u(passed);
-    if ((t & 31) == 0) sPassed[t >> 5] = passed;
-    asm volatile("bar.sync 1, 128;" ::: "memory");          // consumers only (the producer warp has left)
-    if (t == 0) {
-        const unsigned long long tot = (unsigned long long)sPassed[0] + sPassed[1] + sPassed[2] + sPassed[3];
-        if (tot) { atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[set + SET_U_LO]), tot); atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_U_TOT_LO]), tot); }
-    }
-}
-
 // ---- fused re-integration: deIntegrate(old pose) + integrate(new pose) of ONE frame in one pass -------------------
 // The reference re-integrates a frame as two full passes (DepthSensing.cpp:867-895): compactify + stencil for the old pose,
 // alloc + compactify + stencil for the new one.  Each voxel's result depends only on its own state, so running "alloc(new),
@@ -1007,7 +821,7 @@ integrate_tma_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams h
 __global__ void __launch_bounds__(256)
 compactify_dual_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hpOld, const __grid_constant__ BFHashParams hpNew,
                        const __grid_constant__ BFDepthCameraParams cp, const int4* __restrict__ slotInfo, unsigned* ctrs, int set,
-                       unsigned char* __restrict__ listFlags, int4* __restrict__ work, const float2* __restrict__ tiles, int tilesX) {
+                       unsigned char* __restrict__ listFlags, int4* __restrict__ work) {
     const unsigned highWater = ctrs[CTR_HIGH_WATER];
     const unsigned tid = blockIdx.x * blockDim.x + threadIdx.x;
     const int countIdx = set + SET_COUNT, workIdx = set + SET_WORK;
@@ -1015,30 +829,22 @@ compactify_dual_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams
     const unsigned lane = threadIdx.x & 31;
     for (unsigned base = tid - lane; base < highWater; base += stride) {
         const unsigned slot = base + lane;
-        unsigned fl = 0, pr = 0;          // fl: in the old / new frustum (list membership); pr: poses whose stencil can touch the block
+        unsigned fl = 0;                  // bit0: in the old pose's frustum, bit1: in the new pose's
         int4 info = make_int4(0, 0, 0, -1);
         if (slot < highWater) {
             info = __ldcg(&slotInfo[slot]);
             if (info.w >= 0) {
                 I3 b = { info.x, info.y, info.z };
                 fl = (block_in_frustum(hpOld, cp, b) ? 1u : 0u) | (block_in_frustum(hpNew, cp, b) ? 2u : 0u);
-                pr = fl;
-                if (tiles) {
-                    if ((pr & 1u) && !block_can_pass(hpOld, cp, tiles, tilesX, b)) pr &= ~1u;
-                    if ((pr & 2u) && !block_can_pass(hpNew, cp, tiles, tilesX, b)) pr &= ~2u;
-                }
             }
         }
         const unsigned ballot = __ballot_sync(0xffffffffu, fl != 0);
         if (ballot) {
-            const unsigned ballotW = __ballot_sync(0xffffffffu, pr != 0);
             const unsigned nE = __popc(__ballot_sync(0xffffffffu, fl & 1u)) + __popc(__ballot_sync(0xffffffffu, fl & 2u));   // E of both passes
-            const unsigned nP = __popc(__ballot_sync(0xffffffffu, pr & 1u)) + __popc(__ballot_sync(0xffffffffu, pr & 2u));
             unsigned warpBase = 0, workBase = 0;
             if (lane == 0) {
                 warpBase = atomicAdd(&ctrs[countIdx], __popc(ballot));
-                if (ballotW) workBase = atomicAdd(&ctrs[workIdx], __popc(ballotW));
-                if (nE != nP) atomicAdd(&ctrs[set + SET_CULLED], nE - nP);
+                workBase = atomicAdd(&ctrs[workIdx], __popc(ballot));
                 atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_E_TOT_LO]), (unsigned long long)nE);
             }
             warpBase = __shfl_sync(0xffffffffu, warpBase, 0);
@@ -1052,7 +858,7 @@ compactify_dual_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams
                 hd.d_hashCompactified[k] = e;
                 listFlags[k] = (unsigned char)fl;
             }
-            if (pr) work[workBase + __popc(ballotW & ((1u << lane) - 1u))] = make_int4(info.x, info.y, info.z, (int)(slot | (pr << 28)));
+            if (fl) work[workBase + __popc(ballot & ((1u << lane) - 1u))] = make_int4(info.x, info.y, info.z, (int)(slot | (fl << 28)));
         }
     }
 }
@@ -1116,7 +922,7 @@ compactify_multi_kernel(BFHashDataStruct hd, const __grid_constant__ MultiFrusta
             if (lane == 0) {
                 warpBase = atomicAdd(&ctrs[set + SET_COUNT], __popc(ballot));
                 if (b3) base3 = atomicAdd(&ctrs[set + SET_WORK], __popc(b3));
-                if (b2) base2 = atomicAdd(&ctrs[set + SET_CULLED], __popc(b2));      // the batch has no cull: the slot counts quartile-2 items
+                if (b2) base2 = atomicAdd(&ctrs[set + SET_Q2], __popc(b2));
                 if (b1) base1 = atomicAdd(&ctrs[set + SET_Q1], __popc(b1));
                 if (b0) base0 = atomicAdd(&ctrs[set + SET_Q0], __popc(b0));
                 atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_E_TOT_LO]), (unsigned long long)nE);
@@ -1151,12 +957,12 @@ compactify_multi_kernel(BFHashDataStruct hd, const __grid_constant__ MultiFrusta
 
 // truncation test of one voxel against one pose; returns true and the clamped sdf / colour when it passes (.cu:433-463)
 __device__ __forceinline__ bool probe_voxel(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depthImg,
-                                            const uchar4* __restrict__ colorImg, F3 world, float Wf, float Hf, float& sdfOut, uchar4& colOut) {
+                                            const uchar4* __restrict__ colorImg, F3 world, float& sdfOut, uchar4& colOut) {
     const F3 pf = xform(hp.m_rigidTransformInverse, world);
     const float sx = pf.x * cp.fx / pf.z + cp.mx;
     const float sy = pf.y * cp.fy / pf.z + cp.my;
     unsigned px, py;
-    if (!(pixel_index(sx + 0.5f, cp.m_imageWidth, Wf, px) && pixel_index(sy + 0.5f, cp.m_imageHeight, Hf, py))) return false;
+    if (!(pixel_index(sx + 0.5f, cp.m_imageWidth, px) && pixel_index(sy + 0.5f, cp.m_imageHeight, py))) return false;
     const float depth = __ldg(&depthImg[py * cp.m_imageWidth + px]);
     if (!(depth != -INFINITY && depth < hp.m_maxIntegrationDistance)) return false;
     float sdf = depth - pf.z;
@@ -1167,9 +973,7 @@ __device__ __forceinline__ bool probe_voxel(const BFHashParams& hp, const BFDept
     return true;
 }
 
-#ifndef BF_REINT_MINBLOCKS
 #define BF_REINT_MINBLOCKS 8
-#endif
 __global__ void __launch_bounds__(128, BF_REINT_MINBLOCKS)
 reintegrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hpOld, const __grid_constant__ BFHashParams hpNew,
                    const __grid_constant__ BFDepthCameraParams cp, const float* __restrict__ depthImg, const uchar4* __restrict__ colorImg,
@@ -1180,7 +984,6 @@ reintegrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hpO
     const int lx = (int)((4 * t) & 7), ly = (int)(((4 * t) & 63) >> 3), lz = (int)((4 * t) >> 6);
     unsigned passed = 0;
     const bool spec = count < BF_SPEC_BLOCKS;           // see integrate_kernel
-    const float Wf = (float)cp.m_imageWidth, Hf = (float)cp.m_imageHeight;
     int4 wNext = make_int4(0, 0, 0, 0);
     if (blockIdx.x < count) wNext = __ldg(&work[blockIdx.x]);
     for (unsigned b = blockIdx.x; b < count; b += gridDim.x) {
@@ -1200,8 +1003,8 @@ reintegrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hpO
         for (int k = 0; k < 4; ++k) {
             const I3 pi = { bx * BF_SDF_BLOCK_SIZE + lx + k, by * BF_SDF_BLOCK_SIZE + ly, bz * BF_SDF_BLOCK_SIZE + lz };
             const F3 world = voxel_to_world(hpNew, pi);       // both poses of one scene share the voxel size (checked by the host)
-            if ((fl & 1u) && probe_voxel(hpOld, cp, depthImg, colorImg, world, Wf, Hf, sdfD[k], colD[k])) maskD |= 1u << k;
-            if ((fl & 2u) && probe_voxel(hpNew, cp, depthImg, colorImg, world, Wf, Hf, sdfI[k], colI[k])) maskI |= 1u << k;
+            if ((fl & 1u) && probe_voxel(hpOld, cp, depthImg, colorImg, world, sdfD[k], colD[k])) maskD |= 1u << k;
+            if ((fl & 2u) && probe_voxel(hpNew, cp, depthImg, colorImg, world, sdfI[k], colI[k])) maskI |= 1u << k;
         }
         const unsigned mask = maskD | maskI;
         if (mask) {
@@ -1399,7 +1202,7 @@ gc_live_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, con
 // host side
 // ------------------------------------------------------------------------------------------
 static void free_aux(TsdfAux& a) {
-    cudaFree(a.slotInfo); cudaFree(a.ctrs); cudaFree(a.live); cudaFree(a.listFlags); cudaFree(a.work2[0]); cudaFree(a.work2[1]); cudaFree(a.tiles); cudaFree(a.tilesMulti);
+    cudaFree(a.slotInfo); cudaFree(a.ctrs); cudaFree(a.live); cudaFree(a.listFlags); cudaFree(a.work2[0]); cudaFree(a.work2[1]); cudaFree(a.tilesMulti);
     cudaFree(a.slotEpoch); cudaFree(a.workMask); cudaFree(a.workMask2);
     if (a.lane) cudaStreamDestroy(a.lane);
     if (a.evFork) cudaEventDestroy(a.evFork);
@@ -1462,18 +1265,6 @@ static int do_reset(BFHashDataStruct* hd, const BFHashParams* hp) {
 
 static inline int tiles_x(const BFDepthCameraParams* cp) { return (int)((cp->m_imageWidth + BF_TILE - 1) / BF_TILE); }
 static inline int tiles_y(const BFDepthCameraParams* cp) { return (int)((cp->m_imageHeight + BF_TILE - 1) / BF_TILE); }
-static int ensure_tiles(TsdfAux* aux, const BFDepthCameraParams* cp) {
-    const unsigned need = (unsigned)(tiles_x(cp) * tiles_y(cp));
-    if (need <= aux->tilesCap) return 0;
-    if (aux->tiles) { BF_CHECK(cudaStreamSynchronize(g_stream)); BF_CHECK(cudaFree(aux->tiles)); aux->tiles = nullptr; aux->tilesCap = 0; }
-    BF_CHECK(cudaMalloc(&aux->tiles, sizeof(float2) * need));
-    aux->tilesCap = need;
-    return 0;
-}
-// Per-block depth-range cull: OFF by default.  The cull test lengthens the compactify kernels' critical path on every call while the
-// blocks it can prove dead (mostly: looking at
-// depths beyond the integration distance) were cheap for the stencil anyway (their probes exit at the depth test).
-// bfTsdfSetBlockCull(1) or BF_TSDF_CULL=1 switches it on; results are identical either way (tests/test_tsdf_gpu.py).
 static int g_lanes = -1;             // two-lane op replay (bfTsdfRunOps), see "two lanes" below
 // Stencil arithmetic: BF_TSDF_ARITH_FAST (default; tsdf_fast.cu: tolerance contract, what the reference's --use_fast_math build is to
 // its IEEE build) or BF_TSDF_ARITH_EXACT (this file's kernels: bit-identical to the reference's IEEE build and to oracle/tsdf_oracle.c).
@@ -1482,14 +1273,9 @@ static bool arith_fast() {
     if (g_arith < 0) { const char* e = getenv("BF_TSDF_ARITH"); g_arith = (e && (e[0] == 'e' || e[0] == '0')) ? BF_TSDF_ARITH_EXACT : BF_TSDF_ARITH_FAST; }
     return g_arith == BF_TSDF_ARITH_FAST;
 }
-static int g_cull = -1;
-static bool cull_enabled() {
-    if (g_cull < 0) { const char* e = getenv("BF_TSDF_CULL"); g_cull = (e && e[0] == '1') ? 1 : 0; }
-    return g_cull == 1;
-}
 
 // ---- two lanes ---------------------------------------------------------------------------------------------------
-// Front lane = the caller's stream (g_stream): alloc, depth tiles, compactify, GC.  Back lane = aux->lane: the stencils.
+// Front lane = the caller's stream (g_stream): alloc, compactify, GC.  Back lane = aux->lane: the stencils.
 // Inside a bfTsdfRunOps bracket the stencil of op k runs on the back lane while alloc + compactify of op k+1 run on the
 // front lane: they touch disjoint state (hash / heap / slot table / list k+1  vs  work list k / voxels), both are
 // issue-bound at roughly half an SM's capacity, and the stencil is launched with a grid that leaves room for the other.
@@ -1511,35 +1297,22 @@ static int join_lanes(TsdfAux* aux) {
     return 0;
 }
 
-// withTiles: also leave the depth-tile min/max for the stencil's block cull (library sequences only; the reference-named
-// allocCUDA stub has no say over what is integrated afterwards).  zeroParity >= 0: the launch also zeroes that counter set
-// (the one the following compactify fills).
-static int do_alloc(BFHashDataStruct* hd, const BFHashParams* hp, const float* depth, const BFDepthCameraParams* cp, TsdfAux* aux, bool withTiles, int zeroParity,
+// zeroParity >= 0: the launch also zeroes that counter set (the one the following compactify fills).  tilesOut (batch
+// re-integration only): also leave the frame's depth-tile min/max there for the batch cull.
+static int do_alloc(BFHashDataStruct* hd, const BFHashParams* hp, const float* depth, const BFDepthCameraParams* cp, TsdfAux* aux, int zeroParity,
                     AllocEpoch ep = AllocEpoch{nullptr, 0u}, float2* tilesOut = nullptr) {
     dim3 block(BF_TILE, BF_TILE);
     dim3 grid((cp->m_imageWidth + block.x - 1) / block.x, (cp->m_imageHeight + block.y - 1) / block.y);
-    if (withTiles) { int rc = ensure_tiles(aux, cp); if (rc) return rc; }
     if (zeroParity >= 0) { int rc = front_acquire_set(aux, (unsigned)zeroParity); if (rc) return rc; }
     ++g_launchCount;
-    alloc_kernel<<<grid, block, 0, g_stream>>>(*hd, *hp, *cp, depth, aux->slotInfo, aux->ctrs, tilesOut ? tilesOut : (withTiles ? aux->tiles : nullptr),
-                                               zeroParity >= 0 ? set_of((unsigned)zeroParity) : -1, ep);
-    BF_CHECK(cudaGetLastError());
-    return 0;
-}
-static int do_depth_tiles(const BFHashParams* hp, const float* depth, const BFDepthCameraParams* cp, TsdfAux* aux) {
-    int rc = ensure_tiles(aux, cp); if (rc) return rc;
-    dim3 block(BF_TILE, BF_TILE);
-    dim3 grid((cp->m_imageWidth + block.x - 1) / block.x, (cp->m_imageHeight + block.y - 1) / block.y);
-    ++g_launchCount;
-    depth_tiles_kernel<<<grid, block, 0, g_stream>>>(*hp, *cp, depth, aux->tiles);
+    alloc_kernel<<<grid, block, 0, g_stream>>>(*hd, *hp, *cp, depth, aux->slotInfo, aux->ctrs, tilesOut, zeroParity >= 0 ? set_of((unsigned)zeroParity) : -1, ep);
     BF_CHECK(cudaGetLastError());
     return 0;
 }
 
-// useWork: also emit the stencil work list (library sequences); useTiles: aux->tiles describe the depth image the following
-// stencil will read -> entries no voxel of which can pass are left out of the work list.  setZeroed: the preceding launch
-// (alloc_kernel) already zeroed the counter set of the new parity.
-static int do_compactify(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, TsdfAux* aux, bool useWork, bool useTiles, bool setZeroed) {
+// useWork: also emit the stencil work list (library sequences).  setZeroed: the preceding launch (alloc_kernel) already zeroed
+// the counter set of the new parity.
+static int do_compactify(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, TsdfAux* aux, bool useWork, bool setZeroed) {
     aux->parity ^= 1u;
     aux->lastListDual = false;
     const int set = set_of(aux->parity);
@@ -1549,7 +1322,7 @@ static int do_compactify(BFHashDataStruct* hd, const BFHashParams* hp, const BFD
     }
     ++g_launchCount;
     compactify_kernel<<<grid_for((hp->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(*hd, *hp, *cp, aux->slotInfo, aux->ctrs, set,
-                                                                                            useWork ? aux->work2[aux->parity] : nullptr, (useWork && useTiles) ? aux->tiles : nullptr, tiles_x(cp));
+                                                                                            useWork ? aux->work2[aux->parity] : nullptr);
     BF_CHECK(cudaGetLastError());
     if (aux->pipeOpen) BF_CHECK(cudaEventRecord(aux->evList[aux->parity], g_stream));
     return 0;
@@ -1566,21 +1339,15 @@ static int stencil_end(TsdfAux* aux) {
     if (aux->pipeOpen) { BF_CHECK(cudaEventRecord(aux->evStencil[aux->parity], aux->lane)); aux->stencilPending[aux->parity] = true; }
     return 0;
 }
-// Stencil CTAs per SM inside a two-lane bracket.  Capping the stencil at 4-6 CTAs per SM so that alloc CTAs can co-reside slows the
-// stencil by more than the overlap returns; uncapped, the front lane fills the SMs the stencil's last wave frees.
-static int stencil_per_sm() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("BF_TSDF_LANE_STENCIL_PER_SM"); v = e ? atoi(e) : 16; if (v < 1) v = 1; if (v > 16) v = 16; }
-    return v;
-}
+// CTAs per SM of the exact stencils, inside a two-lane bracket too.  Capping the stencil at 4-6 CTAs per SM so that alloc CTAs can
+// co-reside slows the stencil by more than the overlap returns; uncapped, the front lane fills the SMs the stencil's last wave frees.
+static const int kStencilCtasPerSm = 16;
 
 static int do_integrate(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraData* dd, const BFDepthCameraParams* cp,
                         TsdfAux* aux, bool deIntegrate, bool useListCount, unsigned countOverride) {
     const unsigned upper = useListCount ? hp->m_numSDFBlocks : countOverride;
     if (upper == 0) return 0;
     const uchar4* color = reinterpret_cast<const uchar4*>(dd->d_colorData);
-    static int variant = -1;        // BF_TSDF_INTEGRATE=tma selects the TMA-staged variant (measured slower, see DESIGN.md)
-    if (variant < 0) { const char* e = getenv("BF_TSDF_INTEGRATE"); variant = (e && e[0] == 't') ? 1 : 0; }
     const cudaStream_t sb = back_lane(aux);
     int rc = stencil_begin(aux); if (rc) return rc;
     const bool timeIt = g_profile && g_evUsed < kMaxProfiledLaunches;
@@ -1592,21 +1359,15 @@ static int do_integrate(BFHashDataStruct* hd, const BFHashParams* hp, const BFDe
     }
     ++g_launchCount;
     const int set = set_of(aux->parity);
-    if (arith_fast() && variant == 0) {
-        const int4* work = useListCount ? aux->work2[aux->parity] : nullptr;
+    const int4* work = useListCount ? aux->work2[aux->parity] : nullptr;        // the stubs' list (countOverride) has no work list
+    if (arith_fast()) {
         rc = launch_integrate_fast(hd, hp, cp, dd->d_depthData, dd->d_colorData, deIntegrate, useListCount, countOverride, aux->ctrs, aux->live, work, set,
                                    grid_for(upper, fast_stencil_ctas_per_sm(false)), sb);
         if (rc) return rc;
-    } else if (variant == 0) {
-        const int grid = grid_for(upper, aux->pipeOpen ? stencil_per_sm() : 16);
-        const int4* work = useListCount ? aux->work2[aux->parity] : nullptr;        // the stubs' list (countOverride) has no work list
+    } else {
+        const int grid = grid_for(upper, kStencilCtasPerSm);
         if (deIntegrate) integrate_kernel<true><<<grid, 128, 0, sb>>>(*hd, *hp, *cp, dd->d_depthData, color, useListCount ? 1 : 0, countOverride, aux->ctrs, aux->live, work, set);
         else             integrate_kernel<false><<<grid, 128, 0, sb>>>(*hd, *hp, *cp, dd->d_depthData, color, useListCount ? 1 : 0, countOverride, aux->ctrs, aux->live, work, set);
-    } else {
-        const int grid = grid_for(upper, 6);
-        const unsigned* countPtr = useListCount ? live_count_ptr(aux) : nullptr;
-        if (deIntegrate) integrate_tma_kernel<true><<<grid, 160, 0, sb>>>(*hd, *hp, *cp, dd->d_depthData, color, countPtr, countOverride, aux->ctrs, aux->live, set);
-        else             integrate_tma_kernel<false><<<grid, 160, 0, sb>>>(*hd, *hp, *cp, dd->d_depthData, color, countPtr, countOverride, aux->ctrs, aux->live, set);
     }
     BF_CHECK(cudaGetLastError());
     if (timeIt) { BF_CHECK(cudaEventRecord(g_evStop[g_evUsed], sb)); ++g_evUsed; }
@@ -1618,8 +1379,7 @@ int tsdf_lanes_begin(const BFHashDataStruct* hd, const BFHashParams* hp) {
     if (g_lanes < 0) {               // BF_TSDF_LANES=0 / bfTsdfSetLanes(0): everything on the caller's stream
         const char* e = getenv("BF_TSDF_LANES"); g_lanes = (e && e[0] == '0') ? 0 : 1;
     }
-    const char* v = getenv("BF_TSDF_INTEGRATE");
-    if (!g_lanes || (v && v[0] == 't')) return 0;      // the TMA variant walks d_hashCompactified, which the front lane rewrites
+    if (!g_lanes) return 0;
     TsdfAux* aux;
     int rc = get_aux(hd, hp, &aux, true);
     if (rc) return rc;
@@ -1665,17 +1425,14 @@ BF_API int bfTsdfReset(BFHashDataStruct* hd, const BFHashParams* hp) { return do
 
 BF_API int bfTsdfSetLanes(int enable) { const int prev = g_lanes; g_lanes = enable ? 1 : 0; return prev < 0 ? 1 : prev; }
 BF_API int bfTsdfSetArithmetic(int mode) { const int prev = arith_fast() ? BF_TSDF_ARITH_FAST : BF_TSDF_ARITH_EXACT; g_arith = (mode == BF_TSDF_ARITH_EXACT) ? BF_TSDF_ARITH_EXACT : BF_TSDF_ARITH_FAST; return prev; }
-BF_API int bfTsdfSetBlockCull(int enable) { const int prev = cull_enabled() ? 1 : 0; g_cull = enable ? 1 : 0; return prev; }
 
 BF_API int bfTsdfIntegrateFrame(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraData* dd,
                                 const BFDepthCameraParams* cp, int deIntegrate) {
     TsdfAux* aux;
     int rc = get_aux(hd, hp, &aux, true);
     if (rc) return rc;
-    const bool cull = cull_enabled() && dd->d_colorData != nullptr;
-    if (!deIntegrate) { rc = do_alloc(hd, hp, dd->d_depthData, cp, aux, cull, (int)(aux->parity ^ 1u)); if (rc) return rc; }
-    else if (cull)    { rc = front_acquire_set(aux, aux->parity ^ 1u); if (rc) return rc; rc = do_depth_tiles(hp, dd->d_depthData, cp, aux); if (rc) return rc; }
-    rc = do_compactify(hd, hp, cp, aux, true, cull, /*setZeroed=*/!deIntegrate); if (rc) return rc;
+    if (!deIntegrate) { rc = do_alloc(hd, hp, dd->d_depthData, cp, aux, (int)(aux->parity ^ 1u)); if (rc) return rc; }
+    rc = do_compactify(hd, hp, cp, aux, true, /*setZeroed=*/!deIntegrate); if (rc) return rc;
     return do_integrate(hd, hp, dd, cp, aux, deIntegrate != 0, true, 0);
 }
 
@@ -1686,17 +1443,15 @@ BF_API int bfTsdfReintegrateFrame(BFHashDataStruct* hd, const BFHashParams* hpOl
     TsdfAux* aux;
     int rc = get_aux(hd, hpNew, &aux, true);
     if (rc) return rc;
-    if (dd->d_colorData == nullptr) return do_alloc(hd, hpNew, dd->d_depthData, cp, aux, false, -1);     // no colour: neither pass updates a voxel
+    if (dd->d_colorData == nullptr) return do_alloc(hd, hpNew, dd->d_depthData, cp, aux, -1);     // no colour: neither pass updates a voxel
     if (aux->work == nullptr || hpOld->m_virtualVoxelSize != hpNew->m_virtualVoxelSize) return (int)cudaErrorNotSupported;
-    // the tiles are built with the new pose's parameters; both passes may use them only if they accept the same depths
-    const bool cull = cull_enabled() && hpOld->m_maxIntegrationDistance == hpNew->m_maxIntegrationDistance;
-    rc = do_alloc(hd, hpNew, dd->d_depthData, cp, aux, cull, (int)(aux->parity ^ 1u)); if (rc) return rc;
+    rc = do_alloc(hd, hpNew, dd->d_depthData, cp, aux, (int)(aux->parity ^ 1u)); if (rc) return rc;
     aux->parity ^= 1u;
     aux->lastListDual = true;
     const int set = set_of(aux->parity);
     ++g_launchCount;
     compactify_dual_kernel<<<grid_for((hpNew->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(*hd, *hpOld, *hpNew, *cp, aux->slotInfo, aux->ctrs, set, aux->listFlags,
-                                                                                                    aux->work2[aux->parity], cull ? aux->tiles : nullptr, tiles_x(cp));
+                                                                                                    aux->work2[aux->parity]);
     BF_CHECK(cudaGetLastError());
     if (aux->pipeOpen) BF_CHECK(cudaEventRecord(aux->evList[aux->parity], g_stream));
     const cudaStream_t sb = back_lane(aux);
@@ -1714,7 +1469,7 @@ BF_API int bfTsdfReintegrateFrame(BFHashDataStruct* hd, const BFHashParams* hpOl
                                      grid_for(hpNew->m_numSDFBlocks, fast_stencil_ctas_per_sm(true)), sb);
         if (rc) return rc;
     } else {
-        reintegrate_kernel<<<grid_for(hpNew->m_numSDFBlocks, aux->pipeOpen ? stencil_per_sm() : 16), 128, 0, sb>>>(
+        reintegrate_kernel<<<grid_for(hpNew->m_numSDFBlocks, kStencilCtasPerSm), 128, 0, sb>>>(
             *hd, *hpOld, *hpNew, *cp, dd->d_depthData, reinterpret_cast<const uchar4*>(dd->d_colorData), aux->work2[aux->parity], set, aux->ctrs, aux->live);
     }
     BF_CHECK(cudaGetLastError());
@@ -1734,13 +1489,6 @@ static bool batching_on() {
     return g_batching == 1;
 }
 BF_API int bfTsdfSetBatching(int enable) { const int prev = batching_on() ? 1 : 0; g_batching = enable ? 1 : 0; return prev; }
-// Batch cull (compactify_multi_kernel): on by default; BF_TSDF_BATCH_CULL=0 or bfTsdfSetBatchCull(0) switches it off.  Results are identical either way.
-static int g_batchCull = -1;
-static bool batch_cull_on() {
-    if (g_batchCull < 0) { const char* e = getenv("BF_TSDF_BATCH_CULL"); g_batchCull = (e && e[0] == '0') ? 0 : 1; }
-    return g_batchCull == 1;
-}
-BF_API int bfTsdfSetBatchCull(int enable) { const int prev = batch_cull_on() ? 1 : 0; g_batchCull = enable ? 1 : 0; return prev; }
 
 BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraParams* cp, const BFTsdfReintegration* pairs, int numPairs,
                                   const float* const* d_depthFrames, const uint8_t* const* d_colorFrames) {
@@ -1764,8 +1512,7 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
     BFMultiOpDesc desc[BF_MULTI_MAX_OPS];
     fr.nOps = numPairs; fr.voxelSize = hp->m_virtualVoxelSize; fr.truncScale = hp->m_truncScale; fr.truncation = hp->m_truncation;
     fr.tilesX = tiles_x(cp); fr.tilesPerOp = (unsigned)(tiles_x(cp) * tiles_y(cp));
-    const bool cull = batch_cull_on();
-    if (cull && aux->tilesMultiPer < fr.tilesPerOp) {
+    if (aux->tilesMultiPer < fr.tilesPerOp) {
         if (aux->tilesMulti) { BF_CHECK(cudaStreamSynchronize(g_stream)); BF_CHECK(cudaFree(aux->tilesMulti)); aux->tilesMulti = nullptr; aux->tilesMultiPer = 0; }
         BF_CHECK(cudaMalloc(&aux->tilesMulti, sizeof(float2) * (size_t)fr.tilesPerOp * BF_MULTI_MAX_OPS));
         aux->tilesMultiPer = fr.tilesPerOp;
@@ -1781,8 +1528,8 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
         desc[k].depth = d_depthFrames[pairs[k].frame]; desc[k].color = d_colorFrames[pairs[k].frame];
         if (!desc[k].color || !desc[k].depth) return (int)cudaErrorInvalidValue;
         // the first alloc launch also zeroes the counter set the list is about to use
-        rc = do_alloc(hd, &hpNew[k], desc[k].depth, cp, aux, false, k == 0 ? (int)newParity : -1, AllocEpoch{aux->slotEpoch, (aux->batchId << 8) | (unsigned)k},
-                      cull ? aux->tilesMulti + (size_t)k * fr.tilesPerOp : nullptr);
+        rc = do_alloc(hd, &hpNew[k], desc[k].depth, cp, aux, k == 0 ? (int)newParity : -1, AllocEpoch{aux->slotEpoch, (aux->batchId << 8) | (unsigned)k},
+                      aux->tilesMulti + (size_t)k * fr.tilesPerOp);
         if (rc) return rc;
     }
     aux->parity = newParity;
@@ -1791,7 +1538,7 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
     ++g_launchCount;
     compactify_multi_kernel<<<grid_for((hp->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(*hd, fr, *cp, aux->slotInfo, aux->slotEpoch, aux->batchId, aux->ctrs, set,
                                                                                                  aux->listFlags, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots,
-                                                                                                 cull ? aux->tilesMulti : nullptr);
+                                                                                                 aux->tilesMulti);
     BF_CHECK(cudaGetLastError());
     const bool timeIt = g_profile && g_evUsed < kMaxProfiledLaunches;
     if (g_profile) { ++g_profLaunches; g_profFrames += (unsigned long long)numPairs; ++g_profBatchLaunches; g_profBatchFrames += (unsigned long long)numPairs; }
@@ -1851,7 +1598,7 @@ BF_API int bfTsdfGetLastFrameStats(const BFHashDataStruct* hd, unsigned long lon
     BF_CHECK(cudaStreamSynchronize(g_stream));
     out[0] = c[CTR_E];
     const int set = set_of(aux->parity);
-    out[1] = c[set + SET_CULLED];
+    out[1] = 0;
     out[2] = ((unsigned long long)c[set + SET_U_HI] << 32) | c[set + SET_U_LO];
     out[3] = (unsigned long long)c[CTR_HEAP_FAIL] + c[CTR_DROPPED];
     return 0;
@@ -1955,7 +1702,7 @@ BF_API void allocCUDA(BFHashDataStruct* hd, const BFHashParams* hp, const BFDept
     BF_SAFE(get_aux(hd, &g_hashParams, &aux, true));
     BFDepthCameraParams cam = g_camParams;
     cam.m_imageWidth = cp->m_imageWidth; cam.m_imageHeight = cp->m_imageHeight;   // grid follows the argument (.cu:255)
-    BF_SAFE(do_alloc(hd, &g_hashParams, g_bound.d_depthData, &cam, aux, false, -1));
+    BF_SAFE(do_alloc(hd, &g_hashParams, g_bound.d_depthData, &cam, aux, -1));
 }
 
 BF_API void fillDecisionArrayCUDA(BFHashDataStruct* hd, const BFHashParams* hp) {
@@ -1973,7 +1720,7 @@ BF_API unsigned int compactifyHashAllInOneCUDA(BFHashDataStruct* hd, const BFHas
     (void)hp;
     TsdfAux* aux;
     BF_SAFE(get_aux(hd, &g_hashParams, &aux, true));
-    BF_SAFE(do_compactify(hd, &g_hashParams, &g_camParams, aux, false, false, false));
+    BF_SAFE(do_compactify(hd, &g_hashParams, &g_camParams, aux, false, false));
     unsigned res = 0;
     BF_SAFE((int)cudaMemcpyAsync(&res, live_count_ptr(aux), sizeof(unsigned), cudaMemcpyDeviceToHost, g_stream));
     BF_SAFE((int)cudaStreamSynchronize(g_stream));

@@ -48,12 +48,8 @@ struct MultiArgs {
 };
 
 // resident CTAs per SM the kernels are compiled for: the fused pass keeps two poses' probe sets live (<= 64 registers), the others 48
-#ifndef BF_FAST_MINBLOCKS
 #define BF_FAST_MINBLOCKS 10
-#endif
-#ifndef BF_FAST_MINBLOCKS_FUSED
 #define BF_FAST_MINBLOCKS_FUSED 8
-#endif
 
 #ifdef BF_EMU_SEQUENTIAL      // tests/test_tsdf_fast_emulated.py: this source executed on the CPU, one CUDA thread after the other
 __device__ __forceinline__ float rcp_approx(float x) { return 1.0f / x; }
@@ -374,7 +370,7 @@ stencil_fast_kernel(const __grid_constant__ FastArgs a) {
 __global__ void __launch_bounds__(128, BF_FAST_MINBLOCKS_FUSED)
 stencil_multi_kernel(const __grid_constant__ MultiArgs a) {
     // ticket i -> work item: the four cost buckets in order, costliest first (layout: tsdf_shared.cuh)
-    const unsigned n3 = a.ctrs[a.set + SET_WORK], n2 = a.ctrs[a.set + SET_CULLED], n1 = a.ctrs[a.set + SET_Q1], n0 = a.ctrs[a.set + SET_Q0];
+    const unsigned n3 = a.ctrs[a.set + SET_WORK], n2 = a.ctrs[a.set + SET_Q2], n1 = a.ctrs[a.set + SET_Q1], n0 = a.ctrs[a.set + SET_Q0];
     const unsigned e3 = n3, e2 = n3 + n2, e1 = e2 + n1, count = e1 + n0;
     const unsigned t = threadIdx.x;
     if (blockIdx.x == 0 && t == 0) { const unsigned listCount = a.ctrs[a.set + SET_COUNT]; a.listCounterOut[0] = (int)listCount; a.ctrs[CTR_E] = listCount; }

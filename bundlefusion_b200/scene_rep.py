@@ -195,7 +195,7 @@ class CUDASceneRepHashSDF:
         self._bind_stream()
         out = (C.c_ulonglong * 4)()
         capi.check(self.lib.bfTsdfGetLastFrameStats(C.byref(self.m_hashData), out), "bfTsdfGetLastFrameStats")
-        return {"E": out[0], "culled": out[1], "U": out[2], "dropped": out[3]}
+        return {"E": out[0], "U": out[2], "dropped": out[3]}
 
     def runOps(self, ops, depth_frames, color_frames, cam: BFDepthCameraParams):
         """Replay a list of (kind, frame, pose) TSDF operations in ONE library call (bfTsdfRunOps): the re-integration

@@ -207,9 +207,6 @@ int bfTsdfReset(BFHashDataStruct* hashData, const BFHashParams* hashParams);
 #define BF_TSDF_ARITH_FAST 1
 int bfTsdfSetArithmetic(int mode);
 
-/* Per-block depth-range cull of the stencil (default off, see tsdf.cu; results are identical either way -- the cull only skips blocks none
- * of whose voxels can pass the reference's truncation test, .cu:433-449).  Returns the previous setting. */
-int bfTsdfSetBlockCull(int enable);
 /* Two-lane replay inside bfTsdfRunOps (default on): the stencil of operation k runs on a library-owned stream while alloc +
  * compactify of operation k+1 run on the caller's stream; the caller's stream is ordered after all of it on return.  Results are
  * identical either way.  Returns the previous setting. */
@@ -239,16 +236,14 @@ int bfTsdfReintegrateFrame(BFHashDataStruct* hashData, const BFHashParams* hashP
  * k, as in the reference's order.  Fast arithmetic only (bfTsdfSetArithmetic); results are bit-identical to replaying the pairs one by one
  * through bfTsdfReintegrateFrame in fast arithmetic.  hashParams carries the pose-independent parameters and returns holding the last new
  * pose.  d_hashCompactified then holds the union list (its GC flags mark the last pair's new-pose frustum, the list the reference's GC walks).
- * bfTsdfRunOps routes runs of >= 2 pairs here when batching is on (default; BF_TSDF_BATCH=0 / bfTsdfSetBatching(0) replays pair by pair). */
+ * bfTsdfRunOps routes runs of >= 2 pairs here when batching is on (default; BF_TSDF_BATCH=0 / bfTsdfSetBatching(0) replays pair by pair).
+ * Batch cull: while building the union list, a (block, pair, pose) whose voxels provably all fail the truncation test against the pair's frame
+ * (16x16-pixel depth min / max under the block's screen footprint, left behind by the pair's alloc launch; conservative margins) is not handed
+ * to the stencil.  Results are unchanged; E (in-frustum blocks) still counts the culled entries, bfTsdfGetProfileEx out[15] how many were removed. */
 typedef struct BFTsdfReintegration { int32_t frame; float oldPose[16]; float newPose[16]; } BFTsdfReintegration;
 int bfTsdfReintegrateBatch(BFHashDataStruct* hashData, BFHashParams* hashParams, const BFDepthCameraParams* depthCameraParams,
                            const BFTsdfReintegration* pairs, int numPairs, const float* const* d_depthFrames, const uint8_t* const* d_colorFrames);
 int bfTsdfSetBatching(int enable);
-/* Batch cull: while building the union list of a batch, a (block, pair, pose) whose voxels provably all fail the truncation test against the pair's
- * frame (16x16-pixel depth min / max under the block's screen footprint, left behind by the pair's alloc launch; conservative margins) is not
- * handed to the stencil.  Results are identical with it on (default) or off (BF_TSDF_BATCH_CULL=0 / bfTsdfSetBatchCull(0)); E (in-frustum blocks)
- * still counts the culled entries, bfTsdfGetProfileEx out[15] reports how many probes were removed.  Returns the previous setting. */
-int bfTsdfSetBatchCull(int enable);
 
 /* CUDASceneRepHashSDF::garbageCollect (h:110-126) over the last compactified list */
 int bfTsdfGarbageCollect(BFHashDataStruct* hashData, const BFHashParams* hashParams);
@@ -259,7 +254,7 @@ int bfTsdfGetNumOccupiedBlocks(const BFHashDataStruct* hashData, unsigned int* o
 
 /* counters of the last bfTsdfIntegrateFrame, for the roofline arithmetic
  * (SURVEY.md section 8d: U = voxels passing the truncation test, E = in-frustum blocks).
- * out[0]=E, out[1]=block passes the depth-range cull skipped in the last stencil, out[2]=U, out[3]=block inserts dropped since reset
+ * out[0]=E, out[1]=0 (reserved), out[2]=U, out[3]=block inserts dropped since reset
  * (heap exhausted or no free entry inside the probe window; 0 in a sanely sized table).  Synchronises. */
 int bfTsdfGetLastFrameStats(const BFHashDataStruct* hashData, unsigned long long out[4]);
 

@@ -16,7 +16,6 @@ scene.runOps([(0, i, poses[i]) for i in range(B)], dl, cl, cam)
 torch.cuda.synchronize()
 for r in (5, 60, 127):
     scene.integrate(poses[r], dl[r], cl[r], cam)
-    st = scene.getLastFrameStats()
     snap = scene.download()
     E = snap["compactified_count"]
     ent = torch.from_numpy(snap["compactified"][:E].astype(np.int32)).to(dev)           # (E, 8): pos xyz, offset, ptr
@@ -44,5 +43,4 @@ for r in (5, 60, 127):
     # 16-byte piece granularity: thread = 4 consecutive voxels
     q = ok.reshape(E, 128, 4).any(2)
     out["quads_touched"] = float(q.float().mean())
-    out["culled_by_library"] = st["culled"] / max(1, st["E"])
     print(json.dumps(out), flush=True)

@@ -14,6 +14,7 @@ from bundlefusion_b200 import _capi as capi
 from bundlefusion_b200 import synth
 from bundlefusion_b200.scene_rep import CUDASceneRepHashSDF, camera_params, default_hash_params
 from oracle import oracle as orc
+from tests.test_tsdf_gpu import degrade_depth
 from tests.test_tsdf_vs_reference_gpu import compare_states, reference_stream, reintegration_pose
 
 pytestmark = pytest.mark.gpu
@@ -146,12 +147,28 @@ def test_batched_reintegration_equals_pair_by_pair(cuda_device):
     """bfTsdfRunOps with batching (n alloc launches, one union list, one multi-op stencil pass per run of re-integration pairs) against the same
     op list replayed pair by pair, both in fast arithmetic: voxels, block set and heap must be IDENTICAL bit for bit -- the batch changes how
     often a voxel travels, not what happens to it; a block inserted by pair k's alloc stays invisible to the pairs before k."""
+    _batched_vs_pair_by_pair(cuda_device, degraded=False)
+
+
+def test_batched_reintegration_equals_pair_by_pair_degraded_depth(cuda_device):
+    """The same on degraded depth maps (tests/test_tsdf_gpu.py: degrade_depth): they meet the batch's depth-range cull with its adversarial
+    cases, while the pair-by-pair replay has no cull."""
+    _batched_vs_pair_by_pair(cuda_device, degraded=True)
+
+
+def _batched_vs_pair_by_pair(cuda_device, degraded):
     import torch
     W, H = 320, 240
     cam = camera_params(W, H)
-    hp = default_hash_params(num_buckets=100003, num_sdf_blocks=60000)
+    if not degraded:
+        hp = default_hash_params(num_buckets=100003, num_sdf_blocks=60000)
+        frames, dl, cl = _frames(torch, cuda_device, 8, W, H, step=35)
+    else:
+        hp = default_hash_params(num_buckets=100003, num_sdf_blocks=60000, max_integration_distance=2.5)
+        frames = [synth.make_frame(35 * i, W, H) for i in range(8)]
+        degrade_depth(frames)
+        dl, cl = [torch.from_numpy(f[0]).to(cuda_device) for f in frames], [torch.from_numpy(f[1]).to(cuda_device) for f in frames]
     L = capi.lib()
-    frames, dl, cl = _frames(torch, cuda_device, 8, W, H, step=35)
     rng = np.random.default_rng(11)
     ops = [(capi.BF_TSDF_OP_INTEGRATE, i, frames[i][2]) for i in range(6)]
     cur = [f[2] for f in frames]
