@@ -252,6 +252,8 @@ struct Loop {
     Bundler* aheadTarget = nullptr; unsigned aheadLi = 0;
     // stage profile (bfFrameLoopSetProfiling): events at the stage boundaries of a step, elapsed times summed per stage
     bool profile = false; cudaEvent_t stageEv[BF_FRAMELOOP_STAGES + 1] = {}; bool stageHit[BF_FRAMELOOP_STAGES + 1] = {}; double stageMs[BF_FRAMELOOP_STAGES] = {}; unsigned long long profiledSteps = 0;
+    // op log (bfFrameLoopSetOpLog): every TSDF op reconstruct() hands to bfTsdfRunOps, with the turn (step or past-end turn, counted from 0) that issued it
+    bool opLogOn = false; unsigned turn = 0; std::vector<BFTsdfOp> opLog; std::vector<uint32_t> opLogTurn;
 };
 // boundary k = end of stage k - 1 / start of stage k
 static void mark(Loop& L, int k) { if (L.profile && L.stageEv[k]) { cudaEventRecord(L.stageEv[k], stream()); L.stageHit[k] = true; } }
@@ -756,7 +758,9 @@ static int reconstruct(Loop& L, bool gotFrame, unsigned curFrame) {
             memcpy(L.status.transform, ninf, 64);
         }
     }
+    const unsigned turn = L.turn++;
     if (P.reconstructionEnabled) {
+        if (L.opLogOn) { L.opLog.insert(L.opLog.end(), ops.begin(), ops.end()); L.opLogTurn.insert(L.opLogTurn.end(), ops.size(), turn); }
         // inputs of this call that live on the main stream: the frame store (ingest of this frame) -- the poses and the op list are host data
         const bool side = L.overlap && !L.profile && L.tsdfStream;
         cudaStream_t mainStream = stream();
@@ -1108,6 +1112,29 @@ BF_API const BFHashDataStruct* bfFrameLoopGetHashData(const BFFrameLoop* loop) {
     if (!loop) return nullptr;
     join_tsdf(*const_cast<Loop*>(reinterpret_cast<const Loop*>(loop)));          // work the caller queues on the library stream after this call sees the fused model
     return &reinterpret_cast<const Loop*>(loop)->hd;
+}
+BF_API int bfFrameLoopSetOpLog(BFFrameLoop* loop, int enable) {
+    if (!loop) return (int)cudaErrorInvalidValue;
+    Loop& L = *reinterpret_cast<Loop*>(loop);
+    const int prev = L.opLogOn ? 1 : 0;
+    if (enable && !L.opLogOn) { L.opLog.clear(); L.opLogTurn.clear(); }
+    L.opLogOn = enable != 0;
+    return prev;
+}
+BF_API uint32_t bfFrameLoopGetOpLog(const BFFrameLoop* loop, BFTsdfOp* out, uint32_t* turnOfOp, uint32_t maxOps) {
+    if (!loop) return 0;
+    const Loop& L = *reinterpret_cast<const Loop*>(loop);
+    const size_t m = std::min<size_t>(L.opLog.size(), maxOps);
+    if (out) std::copy(L.opLog.begin(), L.opLog.begin() + m, out);
+    if (turnOfOp) std::copy(L.opLogTurn.begin(), L.opLogTurn.begin() + m, turnOfOp);
+    return (uint32_t)L.opLog.size();
+}
+BF_API int bfFrameLoopGetFrame(const BFFrameLoop* loop, uint32_t f, const float** depth, const uint8_t** color) {
+    if (!loop || !depth || !color) return (int)cudaErrorInvalidValue;
+    const Loop& L = *reinterpret_cast<const Loop*>(loop);
+    if (f >= L.numFrames) { set_last_error("bfFrameLoopGetFrame: the frame has not been stepped", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    *depth = L.d_frameDepth[f]; *color = L.d_frameColor[f];
+    return 0;
 }
 BF_API int bfFrameLoopJoin(BFFrameLoop* loop) { return loop ? join_tsdf(*reinterpret_cast<Loop*>(loop)) : (int)cudaErrorInvalidValue; }
 BF_API int bfFrameLoopSetOverlap(BFFrameLoop* loop, int enable) {

@@ -98,6 +98,10 @@ def _bind(L):
     L.bfFrameLoopGetCounters.restype = None
     L.bfFrameLoopSetOverlap.argtypes = [vp, C.c_int]
     L.bfFrameLoopJoin.argtypes = [vp]
+    L.bfFrameLoopSetOpLog.argtypes = [vp, C.c_int]
+    L.bfFrameLoopGetOpLog.argtypes = [vp, C.POINTER(capi.BFTsdfOp), C.POINTER(C.c_uint32), C.c_uint32]
+    L.bfFrameLoopGetOpLog.restype = C.c_uint32
+    L.bfFrameLoopGetFrame.argtypes = [vp, C.c_uint32, C.POINTER(vp), C.POINTER(vp)]
     L.bfFrameLoopSetProfiling.argtypes = [vp, C.c_int]
     L.bfFrameLoopGetStageTimes.argtypes = [vp, C.c_double * 8]
     L.bfFrameLoopGetStageTimes.restype = C.c_ulonglong
@@ -188,6 +192,32 @@ class FrameLoop:
     def join(self) -> None:
         self._bind_stream()
         capi.check(self.lib.bfFrameLoopJoin(self._h), "bfFrameLoopJoin")
+
+    def set_op_log(self, enable: bool) -> bool:
+        """record every TSDF op the loop runs (bfFrameLoopSetOpLog; enabling from off starts an empty log); returns the previous setting"""
+        return bool(self.lib.bfFrameLoopSetOpLog(self._h, 1 if enable else 0))
+
+    def op_log(self):
+        """the recorded ops: (kinds int32 [n], frames int32 [n], poses float32 [n, 4, 4], turns uint32 [n])"""
+        n = int(self.lib.bfFrameLoopGetOpLog(self._h, None, None, 0))
+        ops, turns = (capi.BFTsdfOp * max(1, n))(), np.zeros(max(1, n), np.uint32)
+        m = int(self.lib.bfFrameLoopGetOpLog(self._h, ops, turns.ctypes.data_as(C.POINTER(C.c_uint32)), n))
+        raw = np.frombuffer(ops, np.uint8).reshape(-1, C.sizeof(capi.BFTsdfOp))[:m]
+        words = raw.view(np.int32)
+        return words[:, 0].copy(), words[:, 1].copy(), raw[:, 8:].copy().view(np.float32).reshape(m, 4, 4), turns[:m].copy()
+
+    def frame(self, f: int):
+        """frame f as the loop's frame store holds it (bfFrameLoopGetFrame): (depth float32 [H, W], colour uint8 [H, W, 4]) torch views of the
+        loop's device memory at integration resolution -- no copy, valid while the loop lives"""
+        d, c = C.c_void_p(), C.c_void_p()
+        capi.check(self.lib.bfFrameLoopGetFrame(self._h, int(f), C.byref(d), C.byref(c)), "bfFrameLoopGetFrame")
+        W, H = int(self.params.integrationWidth), int(self.params.integrationHeight)
+
+        class _View:
+            def __init__(self, ptr, shape, typestr):
+                self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "version": 3, "strides": None}
+        t = self._torch
+        return (t.as_tensor(_View(d.value, (H, W), "<f4"), device=self.device), t.as_tensor(_View(c.value, (H, W, 4), "|u1"), device=self.device))
 
     def set_profiling(self, enable: bool) -> None:
         capi.check(self.lib.bfFrameLoopSetProfiling(self._h, 1 if enable else 0), "bfFrameLoopSetProfiling")

@@ -32,6 +32,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "bf_host.h"
 #include "bf_solver.h"
 #include "bf_tsdf.h"
 
@@ -170,6 +171,15 @@ unsigned int bfFrameLoopGetTrajectory(BFFrameLoop* loop, float* h_out, unsigned 
 /* the voxel hash the loop integrates into (caller may read it; bf_tsdf.h) */
 const BFHashDataStruct* bfFrameLoopGetHashData(const BFFrameLoop* loop);
 const BFHashParams* bfFrameLoopGetHashParams(const BFFrameLoop* loop);
+/* Op log (off by default; when off it costs one branch per turn): every BFTsdfOp the loop hands to bfTsdfRunOps -- re-integration items, the
+ * GARBAGE_COLLECT, the INTEGRATE of the current frame -- in order, with the turn that issued it (steps and past-end turns, bfFrameLoopFinish's
+ * included, counted from 0 since bfFrameLoopCreate).  Enabling it from off starts an empty log; returns the previous setting.
+ * bfFrameLoopGetOpLog copies the first min(n, maxOps) ops and turns (either pointer may be NULL) and returns n, the number recorded. */
+int bfFrameLoopSetOpLog(BFFrameLoop* loop, int enable);
+uint32_t bfFrameLoopGetOpLog(const BFFrameLoop* loop, BFTsdfOp* out, uint32_t* turnOfOp, uint32_t maxOps);
+/* Device pointers into the loop's frame store: the integration-resolution depth (float [integrationHeight][integrationWidth]) and colour
+ * (uchar4) of frame f, the images every TSDF op of frame f reads.  Written on the library stream; cudaErrorInvalidValue for a frame not yet stepped. */
+int bfFrameLoopGetFrame(const BFFrameLoop* loop, uint32_t f, const float** depth, const uint8_t** color);
 /* counters for measurement: out[0] frames, out[1] integrations, out[2] re-integrations, out[3] local solves, out[4] global solves,
  * out[5] PCG iterations (global, last solve), out[6] host synchronisations, out[7] keyframes */
 void bfFrameLoopGetCounters(const BFFrameLoop* loop, unsigned long long out[8]);

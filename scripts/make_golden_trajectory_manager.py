@@ -2,7 +2,7 @@
 by oracle/build_ref.py from FL/TrajectoryManager.{h,cpp} + FL/PoseHelper.h with g++) returns on the sessions of
 tests/test_trajectory_manager_reference.py.
 
-    python oracle/build_ref.py && python scripts/make_golden_trajectory_manager.py
+    python oracle/build_ref.py && python scripts/make_golden_trajectory_manager.py < /dev/null
 """
 import ctypes as C
 import os
@@ -12,7 +12,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from tests.test_trajectory_manager_reference import SESSIONS, Recorder, run_session         # noqa: E402
+from tests.test_trajectory_manager_reference import EXTRA_SESSIONS, SESSIONS, Recorder, run_extra_session, run_session         # noqa: E402
 
 
 class Ref:
@@ -51,9 +51,13 @@ class Ref:
 def main():
     names = {"getTopFromDeIntegrateList": 0, "getTopFromIntegrateList": 1, "getTopFromReIntegrateList": 2, "types": 3, "active": 4}
     out = {}
-    for s in range(SESSIONS):
+    for s in list(range(SESSIONS)) + list(EXTRA_SESSIONS):
         rec = Recorder(Ref())
-        run_session(s, [], rec)
+        if isinstance(s, int):
+            run_session(s, [], rec)
+        else:
+            run_extra_session(s, [], rec)
+        p = f"s{s}" if isinstance(s, int) else s
         kinds, found, idx, T, types = [], [], [], [], []
         for name, r in rec.log:
             kinds.append(names[name]); t = np.zeros((2, 16), np.float32)
@@ -68,8 +72,8 @@ def main():
                 if len(r) == 3:
                     t[1] = r[1].reshape(16)
             T.append(t)
-        out[f"s{s}_kind"], out[f"s{s}_found"], out[f"s{s}_idx"] = np.array(kinds, np.int8), np.array(found, np.int8), np.array(idx, np.int32)
-        out[f"s{s}_T"], out[f"s{s}_types"] = np.stack(T), np.array(types, np.int8)
+        out[f"{p}_kind"], out[f"{p}_found"], out[f"{p}_idx"] = np.array(kinds, np.int8), np.array(found, np.int8), np.array(idx, np.int32)
+        out[f"{p}_T"], out[f"{p}_types"] = np.stack(T), np.array(types, np.int8)
         print("session", s, len(kinds), "records")
     path = os.path.join(ROOT, "tests", "golden", "trajectory_manager_reference.npz")
     np.savez_compressed(path, **out)

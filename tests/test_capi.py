@@ -58,6 +58,20 @@ def test_symbol_list_matches_header():
     assert sorted(set(_declared_symbols("bf_marchingcubes.h"))) == sorted(set(capi.MARCHINGCUBES_SYMBOLS))
 
 
+def test_frame_loop_op_log_and_frame_store_accessors():
+    """bfFrameLoopSetOpLog / bfFrameLoopGetOpLog / bfFrameLoopGetFrame are declared, exported and refuse a null loop without a device"""
+    from bundlefusion_b200 import frame_loop
+    names = set(_declared_symbols("bf_frameloop.h"))
+    L = frame_loop._bind(capi.lib())
+    for n in ("bfFrameLoopSetOpLog", "bfFrameLoopGetOpLog", "bfFrameLoopGetFrame"):
+        assert n in names and hasattr(L, n), n
+    assert C.sizeof(capi.BFTsdfOp) == 72
+    assert L.bfFrameLoopSetOpLog(None, 1) == 1                           # cudaErrorInvalidValue
+    assert L.bfFrameLoopGetOpLog(None, None, None, 0) == 0
+    d, c = C.c_void_p(), C.c_void_p()
+    assert L.bfFrameLoopGetFrame(None, 0, C.byref(d), C.byref(c)) == 1
+
+
 def test_solver_grid_policy_override_is_checked_on_the_host():
     """bfSolverSetGridPolicy / bfSolverGetLaunchInfo are exported; an unknown policy is refused without a device and leaves the policy as it was"""
     L = capi.lib()

@@ -5,8 +5,8 @@ the one-CTA Gauss-Newton policy) and 200 frames (about 20 keyframes: the residen
 
 What is checked: the turns before K are bit for bit bfFrameLoopStepPastEnd's; the end solve is bfSolverSolve on the loop's own keyframe problem with the
 reference's end weights, bit for bit; the finished model is the fusion of the returned trajectory: a fresh hash fed every frame at its final pose holds
-the same voxels with the same weights and sdf but for a small, measured fraction (assert_model_is_fusion_of states
-it).  Colour is not compared: the reference's colour de-integration is not an inverse."""
+the same voxels with the same weights and sdf but for a small, measured fraction that allocation history explains (assert_model_is_fusion_of
+states it).  Colour is not compared: the reference's colour de-integration is not an inverse."""
 import ctypes as C
 import math
 
@@ -115,11 +115,15 @@ def fused_voxels(hash_params, raw_frames, trajectory, dev):
 
 
 def assert_model_is_fusion_of(got, want, what):
-    """the loop's model against the fresh fusion of its trajectory.  It is not that fusion bit for bit.  Measured on an H100, as fractions of the
-    voxels with weight > 0: in one model only 1e-5 (43 frames), 1.0e-4 (200 frames), 5e-6 (14-frame scan); another weight 7e-5,
-    2.5e-3, 5e-5; where the weights agree the sdf agrees to 8e-4 m at 43 frames and in the scan, while 1.7e-4 of the 200-frame model's voxels differ by
-    more than 1e-3 m (up to 1.7 cm).  The 43-frame loop run with the bit-exact TSDF arithmetic held the same extra voxels with the same weights, so they
-    do not come from the default arithmetic's rounding; the cause is not established.  The bounds are those figures with headroom."""
+    """the loop's model against the fresh fusion of its trajectory.  It is not that fusion bit for bit, and the cause is allocation history:
+    the model is the exact replay of the TSDF ops the loop ran (tests/test_frame_loop_model_gpu.py, bit for bit), no contribution is stranded
+    on these streams, and integration fills every allocated block in the frustum -- so a frame adds weight to blocks that earlier poses,
+    or later frames, allocated in one model and not (yet) in the other.  The fresh fusion itself moves by the same kind of amount when every
+    block is allocated before the first integration that counts (200 frames: 131 voxels in one model only, 8703 with another weight).
+    Measured on an H100, as fractions of the voxels with weight > 0: in one model only 1e-5 (43 frames), 1.0e-4 (200 frames), 5e-6 (14-frame
+    scan); another weight 7e-5, 2.5e-3, 5e-5; where the weights agree the sdf agrees to 8e-4 m at 43 frames and in the scan, while 1.7e-4 of
+    the 200-frame model's voxels differ by more than 1e-3 m (none against the fusion with every block allocated first).  The bounds are
+    those figures with a factor 2 of headroom."""
     (kg, sg, wg), (kw, sw, ww) = got, want
     assert len(kg) > 10000, (what, len(kg))
     pack = lambda k: (((k[:, 0] + 32768) * 65536 + (k[:, 1] + 32768)) * 65536 + (k[:, 2] + 32768)) * 512 + k[:, 3]
@@ -130,9 +134,9 @@ def assert_model_is_fusion_of(got, want, what):
     far = int((dsdf > SDF_TOL).sum())
     print("%s: %d / %d voxels with weight > 0 (loop / fusion of the trajectory), %d in one model only, %d with another weight, max |delta sdf| %.3g m "
           "where the weights agree (%d above %g m)" % (what, len(kg), len(kw), one_side, int((~same_w).sum()), float(dsdf.max()), far, SDF_TOL))
-    assert one_side <= 5e-4 * len(kw), (what, one_side)
-    assert (~same_w).sum() <= 1e-2 * len(kw), (what, int((~same_w).sum()))
-    assert far <= 1e-3 * len(kw), (what, far)
+    assert one_side <= 2.5e-4 * len(kw), (what, one_side)
+    assert (~same_w).sum() <= 5e-3 * len(kw), (what, int((~same_w).sum()))
+    assert far <= 4e-4 * len(kw), (what, far)
 
 
 class LoopCache:

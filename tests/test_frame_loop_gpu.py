@@ -16,6 +16,25 @@ def rel_pose(T0, T):
     return np.linalg.inv(T0.astype(np.float64)) @ T.astype(np.float64)
 
 
+def canonical_model(loop, dev):
+    """the loop's fused model as oracle.canonical_blocks keys it: block positions and their raw sdf / weight / colour words"""
+    import torch
+    from oracle import oracle as orc
+    hd = loop.lib.bfFrameLoopGetHashData(loop._h).contents
+    hp = loop.lib.bfFrameLoopGetHashParams(loop._h).contents
+    torch.cuda.synchronize(dev)
+
+    def host(ptr, nbytes):
+        class _View:
+            pass
+        v = _View()
+        v.__cuda_array_interface__ = {"shape": (int(nbytes),), "typestr": "|u1", "data": (int(ptr), False), "version": 3, "strides": None}
+        return torch.as_tensor(v, device=dev).cpu().numpy().view(np.int32)
+    n_entries = int(hp.m_hashNumBuckets) * 4
+    return orc.canonical_blocks({"hash": host(hd.d_hash, n_entries * 32).reshape(n_entries, 8),
+                                 "voxels": host(hd.d_SDFBlocks, int(hp.m_numSDFBlocks) * 512 * 12).reshape(-1, 512, 3)})
+
+
 def test_frame_loop_tracks_solves_and_reintegrates(cuda_device):
     import torch
     p = default_params(W, H)
@@ -100,10 +119,11 @@ def test_two_stream_loop_equals_single_stream(cuda_device):
         torch.cuda.synchronize()
         traj = loop.trajectory(25)
         free = loop.heap_free()
-        out.append((sts, traj, free, loop.counters()))
+        out.append((sts, traj, free, loop.counters(), canonical_model(loop, cuda_device)))
         loop.close()
-    (s0, t0, f0, c0), (s1, t1, f1, c1) = out
+    (s0, t0, f0, c0, m0), (s1, t1, f1, c1, m1) = out
     assert f0 == f1 and c0["reintegrations"] == c1["reintegrations"] > 0 and c0["integrations"] == c1["integrations"]
+    assert np.array_equal(m0[0], m1[0]) and np.array_equal(m0[1], m1[1]), "the two-stream loop fused another model"
     for a, b in zip(s0, s1):
         assert a["validTransform"] == b["validTransform"] and a["numReintegrated"] == b["numReintegrated"] and a["localSolved"] == b["localSolved"]
         assert np.array_equal(a["transform"], b["transform"], equal_nan=True)
@@ -112,8 +132,8 @@ def test_two_stream_loop_equals_single_stream(cuda_device):
 
 def test_lookahead_loop_equals_plain_loop(cuda_device):
     """bfFrameLoopStepAhead: the next frame's upload / ingest / SIFT detection / dense cache run on the loop's feature stream while the current frame is
-    matched, solved and fused.  Same kernels, same inputs, destinations fixed one frame early: every status field, the trajectory, the heap and the
-    counters are those of the plain loop -- over two chunk boundaries (where the chunk the next frame belongs to changes), with device and with pinned
+    matched, solved and fused.  Same kernels, same inputs, destinations fixed one frame early: every status field, the trajectory, the heap, the
+    counters and the fused model (canonical voxel words) are those of the plain loop -- over two chunk boundaries (where the chunk the next frame belongs to changes), with device and with pinned
     host frames, with and without the reconstruction stream."""
     import torch
     frames = [synth.make_frame(2 * i, W, H, texture="rich") for i in range(25)]
@@ -133,12 +153,13 @@ def test_lookahead_loop_equals_plain_loop(cuda_device):
             sts.append(loop.step(d, c, *(fr[i + 1] if announce else (None, None))).as_dict())
         loop.join()
         torch.cuda.synchronize()
-        out.append((mode, sts, loop.trajectory(25), loop.heap_free(), loop.counters()))
+        out.append((mode, sts, loop.trajectory(25), loop.heap_free(), loop.counters(), canonical_model(loop, cuda_device)))
         loop.close()
-    _, s0, t0, f0, c0 = out[0]
+    _, s0, t0, f0, c0, m0 = out[0]
     assert c0["local_solves"] == 2 and c0["reintegrations"] > 0
-    for mode, s1, t1, f1, c1 in out[1:]:
+    for mode, s1, t1, f1, c1, m1 in out[1:]:
         assert f0 == f1, mode
+        assert np.array_equal(m0[0], m1[0]) and np.array_equal(m0[1], m1[1]), (mode, "another fused model")
         for k in ("frames", "integrations", "reintegrations", "local_solves", "global_solves", "keyframes"):
             assert c0[k] == c1[k], (mode, k)
         for a, b in zip(s0, s1):

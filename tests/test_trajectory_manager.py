@@ -171,3 +171,120 @@ def test_random_sessions_match_the_restatement(seed):
             if b is not None:
                 tm.confirmIntegration(b[1]); ref.confirmIntegration(b[1])
         same_state(tm, ref, added)
+
+
+def reconstruct_turn(m, ops, max_fixes=10):
+    """the pops of one reintegrate() turn as the frame loop makes them (csrc/frame_loop.cu reconstruct, DepthSensing.cpp:867-899): de-integrate list
+    first, then integrate list, then re-integration list (a pair: de-integrate at the old pose, integrate at the new one); each integration confirmed.
+    Appends (kind, frame, pose) to ops, kind 'D' or 'I'; returns the raw pops."""
+    pops = []
+    for _ in range(max_fixes):
+        r = m.getTopFromDeIntegrateList()
+        if r is not None:
+            pops.append(("de", r)); ops.append(("D", r[1], r[0])); continue
+        r = m.getTopFromIntegrateList()
+        if r is not None:
+            pops.append(("in", r)); ops.append(("I", r[1], r[0])); m.confirmIntegration(r[1]); continue
+        r = m.getTopFromReIntegrateList()
+        if r is not None:
+            pops.append(("re", r)); ops.append(("D", r[2], r[0])); ops.append(("I", r[2], r[1])); m.confirmIntegration(r[2]); continue
+        break
+    return pops
+
+
+def test_frame_invalidated_while_queued_for_reintegration_is_stranded():
+    """A frame whose optimised pose turns -inf while it waits in the re-integration list is popped and skipped
+    (TrajectoryManager.cpp:116-136): it stays of type REINTEGRATION, so the next generateUpdateLists marks it INVALID without queueing a
+    de-integration (cpp:201-210 queues one only for INTEGRATED).  Its old contribution stays in the model; when its pose comes back it is
+    integrated a second time.  The library's class and the restatement agree op for op; the reference's own class is pinned on the same
+    session by test_trajectory_manager_reference.py."""
+    rng = np.random.default_rng(7)
+    poses = np.stack([rand_pose(rng) for _ in range(6)])
+    tm, ref = TrajectoryManager(8, topNActive=8, minPoseDistSqrt=0.0), TrajectoryManagerOracle(8, 8, 0.0)
+    streams = {}
+    for m in (tm, ref):
+        ops = streams.setdefault(id(m), [])
+        for i in range(6):                                               # 1. frames 0-5 integrated
+            m.addFrame(tmod.INTEGRATED, poses[i], i); ops.append(("I", i, poses[i]))
+        m.updateOptimizedTransform(poses, 6); m.generateUpdateLists()
+        assert m.getNumActiveOperations() == 0
+    moved = poses.copy()
+    for i, dx in enumerate((0.4, 0.3, 0.2, 0.1)):                      # 2. frames 0-3 move (0 most): queued for re-integration in that order
+        moved[i, 0, 3] += np.float32(dx)
+    for m in (tm, ref):
+        m.updateOptimizedTransform(moved, 6); m.generateUpdateLists()
+    assert [tm.frameType(i) for i in range(6)] == [tmod.REINTEGRATION] * 4 + [tmod.INTEGRATED] * 2
+    pops = {id(m): reconstruct_turn(m, streams[id(m)], max_fixes=1) for m in (tm, ref)}      # 3. one re-integration: frame 0
+    assert pops[id(tm)][0][1][2] == 0
+    gone = moved.copy(); gone[1:3] = -np.inf                              # 4. frames 1-2 lose their pose while queued
+    for m in (tm, ref):
+        m.updateOptimizedTransform(gone, 6)
+        more = reconstruct_turn(m, streams[id(m)])                       # 5. pop until empty: 1 and 2 are skipped, 3 is re-integrated
+        assert [(k, r[-1]) for k, r in more] == [("re", 3)], more
+        pops[id(m)] += more
+        assert m.getTopFromReIntegrateList() is None
+    assert tm.frameType(1) == tm.frameType(2) == tmod.REINTEGRATION
+    for m in (tm, ref):
+        m.generateUpdateLists()                                          # 6. invalid now, and nothing queued to take them out
+        assert m.getNumActiveOperations() == 0
+    assert tm.frameType(1) == tm.frameType(2) == tmod.INVALID
+    back = moved.copy(); back[1, 1, 3] += np.float32(0.05); back[2, 1, 3] -= np.float32(0.05)
+    for m in (tm, ref):
+        m.updateOptimizedTransform(back, 6); m.generateUpdateLists()      # 7. the poses come back
+        assert m.getNumActiveOperations() == 2
+        while reconstruct_turn(m, streams[id(m)]):                        # 8. drain
+            pass
+        m.generateUpdateLists()
+        assert m.getNumActiveOperations() == 0
+    same_state(tm, ref, 6)
+    a, b = streams[id(tm)], streams[id(ref)]
+    assert len(a) == len(b) and all(x[:2] == y[:2] and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
+    # what that op stream leaves in the model: frames 1 and 2 are never de-integrated and are integrated twice
+    assert not [op for op in a if op[0] == "D" and op[1] in (1, 2)]
+    for f in (1, 2):
+        ins = [op[2] for op in a if op[0] == "I" and op[1] == f]
+        assert len(ins) == 2 and np.array_equal(ins[0], poses[f]) and np.array_equal(ins[1], back[f])
+    contributions = {}
+    for k, f, T in a:
+        lst = contributions.setdefault(f, [])
+        if k == "I":
+            lst.append(T)
+        else:
+            hit = [j for j, U in enumerate(lst) if np.array_equal(U, T)]
+            assert hit, (f, "de-integration of a contribution that is not in the model")
+            lst.pop(hit[0])
+    final = tm.getOptimizedTransforms()
+    for f in range(6):
+        want = 2 if f in (1, 2) else 1
+        assert len(contributions[f]) == want and np.array_equal(contributions[f][-1], final[f]), f
+
+
+def test_reintegration_list_of_invalid_frames_only_returns_a_non_finite_pose():
+    """Every frame left in the re-integration list has lost its pose: the pop still returns 1 (cpp:116-136), with the last skipped frame's index,
+    its integrated pose as the old pose and newT = -inf; the frame loop then queues DEINTEGRATE(old) and INTEGRATE(-inf) for it."""
+    rng = np.random.default_rng(8)
+    poses = np.stack([rand_pose(rng) for _ in range(3)])
+    tm, ref = TrajectoryManager(4, topNActive=4, minPoseDistSqrt=0.0), TrajectoryManagerOracle(4, 4, 0.0)
+    moved = poses.copy(); moved[:, 2, 3] += np.float32([0.3, 0.2, 0.1])
+    gone = np.full_like(poses, -np.inf)
+    for m in (tm, ref):
+        for i in range(3):
+            m.addFrame(tmod.INTEGRATED, poses[i], i)
+        m.updateOptimizedTransform(poses, 3); m.generateUpdateLists()
+        m.updateOptimizedTransform(moved, 3); m.generateUpdateLists()
+        assert m.getNumActiveOperations() == 3
+        m.updateOptimizedTransform(gone, 3)
+    a, b = tm.getTopFromReIntegrateList(), ref.getTopFromReIntegrateList()
+    same_pop(a, b)
+    old, new, idx = a
+    assert idx == 2 and np.array_equal(old, poses[2]) and np.all(np.isneginf(new))
+    assert tm.getNumActiveOperations() == 0 and tm.getTopFromReIntegrateList() is None
+    ops = []
+    tm.confirmIntegration(idx); ref.confirmIntegration(idx)
+    same_state(tm, ref, 3)
+    assert tm.frameType(2) == tmod.INTEGRATED and [tm.frameType(i) for i in (0, 1)] == [tmod.REINTEGRATION] * 2
+    for m in (tm, ref):
+        m.generateUpdateLists()                                          # the -inf frame 2 is INTEGRATED: de-integrated again at its old pose
+        ops.append(m.getTopFromDeIntegrateList())
+    same_pop(ops[0], ops[1])
+    assert ops[0][1] == 2 and np.array_equal(ops[0][0], poses[2])

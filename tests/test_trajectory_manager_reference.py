@@ -126,11 +126,81 @@ def run_session(seed, impls, ref):
             assert m.getNumActiveOperations() == active, (seed, frame)
 
 
+EXTRA_SESSIONS = ("stranded", "all_lost")
+
+
+def run_extra_session(name, impls, ref):
+    """Two scripted sessions around a frame that loses its pose while it waits in the re-integration list.  "stranded": frames 0-5 integrated,
+    0-3 moved (queued 0, 1, 2, 3), one pop, frames 1-2 set to -inf, pops until empty, generateUpdateLists, 1-2 finite again, drain -- 1 and 2
+    are never de-integrated and are integrated a second time.  "all_lost": every queued frame set to -inf; the pop returns the last one with
+    newT = -inf."""
+    rng = np.random.default_rng(900 + EXTRA_SESSIONS.index(name))
+    n = 6 if name == "stranded" else 3
+    made = [make(8, 8, 0.0) for make in impls]
+    ref.create(8, 8, 0.0)
+    everyone = made + [ref]
+    poses = np.stack([rand_pose(rng) for _ in range(n)])
+
+    def each(fn):
+        for m in everyone:
+            fn(m)
+
+    def check(what):
+        types, active = ref.types(n), ref.active()
+        for m in made:
+            mine = [m.frameType(i) for i in range(n)] if hasattr(m, "frameType") else [m.frames[i].type for i in range(n)]
+            assert mine == list(types) and m.getNumActiveOperations() == active, (name, what)
+
+    def pop(limit):
+        for _ in range(limit):
+            for kind in ("getTopFromDeIntegrateList", "getTopFromIntegrateList", "getTopFromReIntegrateList"):
+                b = getattr(ref, kind)()
+                for m in made:
+                    assert same_pop(getattr(m, kind)(), b), (name, kind)
+                if b is not None:
+                    break
+            if b is None:
+                return
+            new = b[1] if kind == "getTopFromReIntegrateList" else b[0]
+            if kind != "getTopFromDeIntegrateList" and not np.isneginf(new[0, 0]):
+                each(lambda m: m.confirmIntegration(b[-1]))
+            check(kind)
+
+    for i in range(n):
+        each(lambda m: m.addFrame(0, poses[i], i))
+    each(lambda m: m.updateOptimizedTransform(poses, n)); each(lambda m: m.generateUpdateLists())
+    moved = poses.copy()
+    for i, dx in enumerate((0.4, 0.3, 0.2, 0.1)[:min(4, n)]):
+        moved[i, 0, 3] += np.float32(dx)
+    each(lambda m: m.updateOptimizedTransform(moved, n)); each(lambda m: m.generateUpdateLists())
+    check("queued")
+    gone = moved.copy()
+    if name == "stranded":
+        pop(1)
+        gone[1:3] = -np.inf
+    else:
+        gone[:] = -np.inf
+    each(lambda m: m.updateOptimizedTransform(gone, n))
+    pop(20)
+    each(lambda m: m.generateUpdateLists())
+    check("invalidated")
+    pop(20)
+    back = moved.copy()
+    if name == "stranded":
+        back[1, 1, 3] += np.float32(0.05); back[2, 1, 3] -= np.float32(0.05)
+    each(lambda m: m.updateOptimizedTransform(back, n)); each(lambda m: m.generateUpdateLists())
+    check("back")
+    pop(20)
+    each(lambda m: m.generateUpdateLists())
+    check("drained")
+
+
 def load_log(g, s):
     names = ["getTopFromDeIntegrateList", "getTopFromIntegrateList", "getTopFromReIntegrateList", "types", "active"]
     log = []
-    kinds, found, idx, T = g[f"s{s}_kind"], g[f"s{s}_found"], g[f"s{s}_idx"], g[f"s{s}_T"]
-    types, tpos = g[f"s{s}_types"], 0
+    p = f"s{s}" if isinstance(s, int) else s
+    kinds, found, idx, T = g[f"{p}_kind"], g[f"{p}_found"], g[f"{p}_idx"], g[f"{p}_T"]
+    types, tpos = g[f"{p}_types"], 0
     for k in range(len(kinds)):
         name = names[kinds[k]]
         if name == "types":
@@ -156,3 +226,21 @@ def test_library_and_restatement_replay_the_reference_sessions():
         assert rp.pos == len(log)
         ops += sum(1 for name, r in log if name.startswith("get") and r is not None)
     assert ops > 1000
+
+
+def test_library_and_restatement_replay_the_reference_on_a_frame_lost_while_queued():
+    """the reference's own class on the two scripted sessions of run_extra_session: what it pops, its frame types and queue sizes after every
+    pop, replayed against the library's class and the restatement"""
+    g = np.load(GOLDEN)
+    for name in EXTRA_SESSIONS:
+        log = load_log(g, name)
+        rp = Replay(log)
+        run_extra_session(name, [TrajectoryManager, TrajectoryManagerOracle], rp)
+        assert rp.pos == len(log), name
+    stranded = load_log(g, "stranded")
+    re_pops = [r for name, r in stranded if name == "getTopFromReIntegrateList" and r is not None]
+    assert [r[2] for r in re_pops] == [0, 3]                              # frames 1 and 2 were skipped, never popped
+    assert not [r for name, r in stranded if name == "getTopFromDeIntegrateList" and r is not None]
+    assert sorted(r[1] for name, r in stranded if name == "getTopFromIntegrateList" and r is not None) == [1, 2]
+    lost = [r for name, r in load_log(g, "all_lost") if name == "getTopFromReIntegrateList" and r is not None]
+    assert lost[0][2] == 2 and np.all(np.isneginf(lost[0][1]))

@@ -248,3 +248,58 @@ def test_dense_grid_config0(oracle_lib):
     t = w > 0
     np.testing.assert_allclose(sdf[t], 2.0 - z[t], atol=2e-6)
     assert np.all(np.abs(sdf[t]) < 0.06 + 0.02 * 2.0)
+
+
+@pytest.mark.parametrize("frame_idx", [100, 200])
+def test_allocation_history_widens_the_integrated_voxel_set(oracle_lib, frame_idx):
+    """integrate(P1), deIntegrate(P1), integrate(P2) is not integrate(P2) on a fresh hash: de-integration clears P1's voxels but not its blocks
+    (GC frees a block only once it is visited with no weight left), and integration fills every allocated block in the frustum, not only the
+    blocks P2's rays allocate.  So the history holds weight in voxels the fresh hash does not have -- every one of them in a block the fresh
+    hash never allocated -- while every block both allocated holds the same voxel words.  This is why a re-integrated model differs from a
+    fresh fusion of its final poses."""
+    W, H = 160, 120
+    cam = camera_params(W, H)
+    hp = small_params()
+    depth, color, P1 = synth.make_frame(frame_idx, W, H)
+    P2 = (synth.se3_exp(np.array([0.01, -0.02, 0.015]), np.array([0.03, -0.02, 0.04])) @ P1.astype(np.float64)).astype(F)
+    P2[3] = [0, 0, 0, 1]
+    hist, fresh = orc.OracleSceneRepHashSDF(hp), orc.OracleSceneRepHashSDF(hp)
+    hist.integrate(P1, depth, color, cam)
+    hist.deIntegrate(P1, depth, color, cam)
+    assert np.all(hist.voxels == 0)
+    hist.integrate(P2, depth, color, cam)
+    fresh.integrate(P2, depth, color, cam)
+    hb, hv = orc.canonical_blocks(hist.download())
+    fb, fv = orc.canonical_blocks(fresh.download())
+    key = lambda b: [tuple(x) for x in b]
+    fset = set(key(fb))
+    in_fresh = np.array([k in fset for k in key(hb)])
+    assert in_fresh.sum() == len(fb)                                     # the history allocated every block the fresh hash did ...
+    np.testing.assert_array_equal(hv[in_fresh], fv)                       # ... and those hold the same voxel words
+    hw = hv[..., 1].view(F)
+    extra = (hw > 0) & ~in_fresh[:, None]
+    assert extra.sum() > 0                                                # weight the fresh hash does not have, all in blocks it never allocated
+    assert int((hw > 0).sum()) == int((fv[..., 1].view(F) > 0).sum()) + int(extra.sum())
+
+
+def test_integrate_at_a_non_finite_pose_changes_no_voxel_and_gc_returns_what_it_allocated(oracle_lib):
+    """the frame loop can issue an INTEGRATE at newT = -inf (every frame left in the re-integration list lost its pose): the inverse pose is NaN,
+    the ray walk inserts a few blocks at meaningless positions, the NaN frustum test passes every block, no voxel passes the truncation test, and
+    the garbage collection of the same turn -- over that all-blocks list -- frees exactly the blocks the call inserted"""
+    W, H = 160, 120
+    cam = camera_params(W, H)
+    hp = small_params()
+    depth, color, T = synth.make_frame(5, W, H)
+    o = orc.OracleSceneRepHashSDF(hp)
+    o.integrate(T, depth, color, cam)
+    before = orc.canonical_blocks(o.download())
+    before = (before[0].copy(), before[1].copy())
+    free0 = o.getHeapFreeCount()
+    o.integrate(np.full((4, 4), -np.inf, F), depth, color, cam)
+    assert o.last_U == 0 and o.getHeapFreeCount() < free0
+    o.garbageCollect()
+    after = orc.canonical_blocks(o.download())
+    assert o.getHeapFreeCount() == free0
+    np.testing.assert_array_equal(after[0], before[0])
+    np.testing.assert_array_equal(after[1], before[1])
+    orc.check_hash_invariants(o.download(), hp)
