@@ -72,17 +72,19 @@ struct TsdfAux {
     const void* owner[3] = { nullptr, nullptr, nullptr };   // the caller's d_SDFBlocks / d_heap / d_hashCompactified: the key (d_hash) can be
                                                             // recycled by an allocator for another table; all four together identify one
 };
-// launch accounting + optional CUDA-event timing of the integrate / de-integrate stencil (bench.py's roofline line)
+// launch accounting + optional CUDA-event timing of the stencil launches (bench.py's roofline line)
 unsigned long long g_launchCount = 0;
-static bool g_profile = false;
-static std::vector<cudaEvent_t> g_evStart, g_evStop;
-static size_t g_evUsed = 0;
-static unsigned long long g_profLaunches = 0;
-static unsigned long long g_profFrames = 0;
-static unsigned long long g_profBatchLaunches = 0, g_profBatchFrames = 0;
-static std::vector<unsigned char> g_evIsBatch;
-static unsigned long long* g_ktime = nullptr;        // [kMaxProfiledLaunches][2] in-kernel %globaltimer brackets of the profiled batch launches      // frame images the profiled stencil launches read (a batch launch reads one per pair)
 static const size_t kMaxProfiledLaunches = 16384;
+struct TimedLaunch { cudaEvent_t start, stop; bool batch; };
+static struct StencilProfile {
+    bool on = false;
+    std::vector<TimedLaunch> ev;     // [0, used): the launches timed since the last reset; the events are reused
+    size_t used = 0;
+    unsigned long long launches = 0, frames = 0;             // stencil launches and the frame images they read (a batch launch reads one per pair)
+    unsigned long long batchLaunches = 0, batchFrames = 0;   // the batch launches among them
+    unsigned long long* ktime = nullptr;                     // [kMaxProfiledLaunches][2] in-kernel %globaltimer brackets of the timed batch launches
+    void reset() { used = 0; launches = frames = batchLaunches = batchFrames = 0; }
+} g_prof;
 
 static std::mutex g_auxMutex;
 static std::map<const void*, TsdfAux> g_aux;
@@ -711,26 +713,92 @@ __device__ __forceinline__ void update_voxel(const BFHashParams& hp, float sdf, 
     wSdf = __float_as_uint(nSdf); wWeight = __float_as_uint(nW); wColor = nColor;
 }
 
-template <bool kDeIntegrate>
-__global__ void __launch_bounds__(128)
-integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp,
-                 const float* __restrict__ depthImg, const uchar4* __restrict__ colorImg,
-                 int useListCount, unsigned countOverride, unsigned* ctrs, int* __restrict__ live,
-                 const int4* __restrict__ work, int set) {
-    const unsigned* countPtr = useListCount ? ctrs + set + SET_COUNT : nullptr;
-    const unsigned* workCountPtr = ctrs + set + SET_WORK;
-    // `work` (from the library's own compactify): one 16-byte item per list entry; without it (reference-named stubs, whose
-    // list may come from anywhere) the kernel walks d_hashCompactified itself.
-    const unsigned listCount = countPtr ? *countPtr : countOverride;
-    const unsigned count = work ? *workCountPtr : listCount;
+// truncation test of one voxel against one pose; returns true and the clamped sdf / colour when it passes (.cu:433-463)
+__device__ __forceinline__ bool probe_voxel(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depthImg,
+                                            const uchar4* __restrict__ colorImg, F3 world, float& sdfOut, uchar4& colOut) {
+    const F3 pf = xform(hp.m_rigidTransformInverse, world);
+    const float sx = pf.x * cp.fx / pf.z + cp.mx;
+    const float sy = pf.y * cp.fy / pf.z + cp.my;
+    unsigned px, py;
+    if (!(pixel_index(sx + 0.5f, cp.m_imageWidth, px) && pixel_index(sy + 0.5f, cp.m_imageHeight, py))) return false;
+    const float depth = __ldg(&depthImg[py * cp.m_imageWidth + px]);
+    if (!(depth != -INFINITY && depth < hp.m_maxIntegrationDistance)) return false;
+    float sdf = depth - pf.z;
+    const float trunc = truncation(hp, depth);
+    if (!(fabsf(sdf) < trunc)) return false;
+    sdfOut = (sdf >= 0.0f) ? fminf(trunc, sdf) : fmaxf(-trunc, sdf);
+    colOut = __ldg(&colorImg[py * cp.m_imageWidth + px]);
+    return true;
+}
+
+// One SDF block: 128 threads, 4 x-consecutive voxels (48 B = three 16-byte vectors) per thread; l = the thread's first voxel in the block.
+// MODE 0: integrate with pose A, 1: de-integrate with pose A, 2: a fused re-integration pair -- per voxel, de-integrate with pose A (the old
+// one), then integrate with pose B (the new one).  Outside MODE 2, hpB is a copy of hpA.  fl: bit0 pose A can touch this block, bit1 pose B can.
+// spec: load the voxel quad before the probes (see integrate_kernel).
+template <int MODE>
+__device__ __forceinline__ void process_block(const BFHashDataStruct& hd, const BFHashParams& hpA, const BFHashParams& hpB, const BFDepthCameraParams& cp,
+                                              const float* __restrict__ depthImg, const uchar4* __restrict__ colorImg, int* __restrict__ live,
+                                              unsigned t, I3 l, bool spec, int bx, int by, int bz, unsigned ptr, unsigned fl, unsigned& passed) {
+    if (colorImg == nullptr) return;                    // without colour nothing passes (.cu:441-448)
+    uint4* const vp = reinterpret_cast<uint4*>(hd.d_SDFBlocks + (size_t)ptr) + 3 * t;   // 48 B per thread, 16-B aligned
+    VoxelQuad q;
+    if (spec) { q.a = vp[0]; q.b = vp[1]; q.c = vp[2]; }
+    float sdfA[4], sdfB[4];
+    uchar4 colA[4], colB[4];
+    unsigned maskA = 0, maskB = 0;
+    int liveDelta = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const I3 pi = { bx * BF_SDF_BLOCK_SIZE + l.x + k, by * BF_SDF_BLOCK_SIZE + l.y, bz * BF_SDF_BLOCK_SIZE + l.z };
+        const F3 world = voxel_to_world(hpB, pi);       // both poses of a pair share the voxel size (checked by the host)
+        if ((fl & 1u) && probe_voxel(hpA, cp, depthImg, colorImg, world, sdfA[k], colA[k])) maskA |= 1u << k;
+        if (MODE == 2 && (fl & 2u) && probe_voxel(hpB, cp, depthImg, colorImg, world, sdfB[k], colB[k])) maskB |= 1u << k;
+    }
+    const unsigned mask = maskA | maskB;
+    if (mask) {
+        if (!spec) { q.a = vp[0]; q.b = vp[1]; q.c = vp[2]; }
+        if (maskA & 1u) update_voxel<MODE != 0>(hpA, sdfA[0], colA[0], q.a.x, q.a.y, q.a.z, liveDelta);
+        if (maskB & 1u) update_voxel<false>(hpB, sdfB[0], colB[0], q.a.x, q.a.y, q.a.z, liveDelta);
+        if (maskA & 2u) update_voxel<MODE != 0>(hpA, sdfA[1], colA[1], q.a.w, q.b.x, q.b.y, liveDelta);
+        if (maskB & 2u) update_voxel<false>(hpB, sdfB[1], colB[1], q.a.w, q.b.x, q.b.y, liveDelta);
+        if (maskA & 4u) update_voxel<MODE != 0>(hpA, sdfA[2], colA[2], q.b.z, q.b.w, q.c.x, liveDelta);
+        if (maskB & 4u) update_voxel<false>(hpB, sdfB[2], colB[2], q.b.z, q.b.w, q.c.x, liveDelta);
+        if (maskA & 8u) update_voxel<MODE != 0>(hpA, sdfA[3], colA[3], q.c.y, q.c.z, q.c.w, liveDelta);
+        if (maskB & 8u) update_voxel<false>(hpB, sdfB[3], colB[3], q.c.y, q.c.z, q.c.w, liveDelta);
+        // write back only the 16-byte pieces that contain an updated voxel
+        // words: v0 = a.xyz | v1 = a.w b.xy | v2 = b.zw c.x | v3 = c.yzw
+        if (mask & 0x3u) vp[0] = q.a;
+        if (mask & 0x6u) vp[1] = q.b;
+        if (mask & 0xCu) vp[2] = q.c;
+        passed += __popc(maskA) + __popc(maskB);
+    }
+    // live-voxel bookkeeping for O(E) garbage collection: one RED per warp, only when a weight crossed zero
+    if (__any_sync(0xffffffffu, liveDelta != 0)) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) liveDelta += __shfl_xor_sync(0xffffffffu, liveDelta, o);
+        if ((t & 31) == 0 && liveDelta != 0) atomicAdd(&live[ptr / BF_SDF_BLOCK_VOXELS], liveDelta);
+    }
+}
+
+// The bit-exact stencil, MODE as process_block's.  Persistent grid: each CTA walks the list with stride gridDim.x; the list length is read
+// from device memory (useListCount) or given (countOverride).  `work` (from the library's own compactify): one 16-byte item per list entry;
+// without it (MODE 0 / 1 of the reference-named stubs, whose list may come from anywhere) the kernel walks d_hashCompactified itself.
+#define BF_REINT_MINBLOCKS 8
+template <int MODE>
+__global__ void __launch_bounds__(128, MODE == 2 ? BF_REINT_MINBLOCKS : 0)     // 0: no minimum
+integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hpA, const __grid_constant__ BFHashParams hpB,
+                 const __grid_constant__ BFDepthCameraParams cp, const float* __restrict__ depthImg, const uchar4* __restrict__ colorImg,
+                 int useListCount, unsigned countOverride, unsigned* ctrs, int* __restrict__ live, const int4* __restrict__ work, int set) {
+    const bool listed = MODE == 2 || work != nullptr;
+    const unsigned listCount = useListCount ? ctrs[set + SET_COUNT] : countOverride;
+    const unsigned count = listed ? ctrs[set + SET_WORK] : listCount;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
-        if (countPtr) { hd.d_hashCompactifiedCounter[0] = (int)listCount; ctrs[CTR_E] = listCount; }
-        if (!work) atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_E_TOT_LO]), (unsigned long long)listCount);
+        if (useListCount) { hd.d_hashCompactifiedCounter[0] = (int)listCount; ctrs[CTR_E] = listCount; }
+        if (!listed) atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_E_TOT_LO]), (unsigned long long)listCount);   // else counted by compactify
     }
     const unsigned t = threadIdx.x;
-    const unsigned W = cp.m_imageWidth, H = cp.m_imageHeight;
     // local voxel coordinates of this thread's first voxel: i = 4t -> x = (4t)%8, y = (4t%64)/8, z = 4t/64
-    const int lx = (int)((4 * t) & 7), ly = (int)(((4 * t) & 63) >> 3), lz = (int)((4 * t) >> 6);
+    const I3 l = { (int)((4 * t) & 7), (int)(((4 * t) & 63) >> 3), (int)((4 * t) >> 6) };
     unsigned passed = 0;
     // Latency, not bandwidth, bounds this kernel while the list is short (a few thousand blocks: each warp walks a dependent
     // chain work item -> projection -> depth gather -> voxel load -> store).  Below BF_SPEC_BLOCKS list entries the voxel quad is
@@ -739,68 +807,22 @@ integrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, c
     // keeps the long-list regime at ~80 % of the roof.  The next work item is prefetched either way.
     const bool spec = count < BF_SPEC_BLOCKS;
     int4 wNext = make_int4(0, 0, 0, 0);
-    if (work && blockIdx.x < count) wNext = __ldg(&work[blockIdx.x]);
+    if (listed && blockIdx.x < count) wNext = __ldg(&work[blockIdx.x]);
 
     for (unsigned b = blockIdx.x; b < count; b += gridDim.x) {
         int bx, by, bz;
-        unsigned ptr;
-        if (work) {
+        unsigned ptr, fl = 1u;
+        if (listed) {
             const int4 w = wNext;
             if (b + gridDim.x < count) wNext = __ldg(&work[b + gridDim.x]);
             bx = w.x; by = w.y; bz = w.z; ptr = ((unsigned)w.w & 0x0FFFFFFFu) * BF_SDF_BLOCK_VOXELS;
+            if (MODE == 2) fl = (unsigned)w.w >> 28;
         } else {
             const BFHashEntry* ep = &hd.d_hashCompactified[b];
             bx = __ldg(&ep->pos[0]); by = __ldg(&ep->pos[1]); bz = __ldg(&ep->pos[2]);
             ptr = (unsigned)__ldg(&ep->ptr);
         }
-
-        uint4* const vp = reinterpret_cast<uint4*>(hd.d_SDFBlocks + (size_t)ptr) + 3 * t;   // 48 B per thread, 16-B aligned
-        VoxelQuad q;
-        if (spec) { q.a = vp[0]; q.b = vp[1]; q.c = vp[2]; }
-        float sdfv[4];
-        uchar4 colv[4];
-        unsigned mask = 0;
-        int liveDelta = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const I3 pi = { bx * BF_SDF_BLOCK_SIZE + lx + k, by * BF_SDF_BLOCK_SIZE + ly, bz * BF_SDF_BLOCK_SIZE + lz };
-            const F3 pf = xform(hp.m_rigidTransformInverse, voxel_to_world(hp, pi));
-            const float sx = pf.x * cp.fx / pf.z + cp.mx;
-            const float sy = pf.y * cp.fy / pf.z + cp.my;
-            unsigned px, py;
-            if (pixel_index(sx + 0.5f, W, px) && pixel_index(sy + 0.5f, H, py) && colorImg != nullptr) {
-                const float depth = __ldg(&depthImg[py * W + px]);
-                if (depth != -INFINITY && depth < hp.m_maxIntegrationDistance) {
-                    float sdf = depth - pf.z;
-                    const float trunc = truncation(hp, depth);
-                    if (fabsf(sdf) < trunc) {
-                        sdf = (sdf >= 0.0f) ? fminf(trunc, sdf) : fmaxf(-trunc, sdf);
-                        sdfv[k] = sdf;
-                        colv[k] = __ldg(&colorImg[py * W + px]);
-                        mask |= 1u << k;
-                    }
-                }
-            }
-        }
-        if (mask) {
-            if (!spec) { q.a = vp[0]; q.b = vp[1]; q.c = vp[2]; }
-            if (mask & 1u) update_voxel<kDeIntegrate>(hp, sdfv[0], colv[0], q.a.x, q.a.y, q.a.z, liveDelta);
-            if (mask & 2u) update_voxel<kDeIntegrate>(hp, sdfv[1], colv[1], q.a.w, q.b.x, q.b.y, liveDelta);
-            if (mask & 4u) update_voxel<kDeIntegrate>(hp, sdfv[2], colv[2], q.b.z, q.b.w, q.c.x, liveDelta);
-            if (mask & 8u) update_voxel<kDeIntegrate>(hp, sdfv[3], colv[3], q.c.y, q.c.z, q.c.w, liveDelta);
-            // write back only the 16-byte pieces that contain an updated voxel
-            // words: v0 = a.xyz | v1 = a.w b.xy | v2 = b.zw c.x | v3 = c.yzw
-            if (mask & 0x3u) vp[0] = q.a;
-            if (mask & 0x6u) vp[1] = q.b;
-            if (mask & 0xCu) vp[2] = q.c;
-            passed += __popc(mask);
-        }
-        // live-voxel bookkeeping for O(E) garbage collection: one RED per warp, only when a weight crossed zero
-        if (__any_sync(0xffffffffu, liveDelta != 0)) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) liveDelta += __shfl_xor_sync(0xffffffffu, liveDelta, o);
-            if ((t & 31) == 0 && liveDelta != 0) atomicAdd(&live[ptr / BF_SDF_BLOCK_VOXELS], liveDelta);
-        }
+        process_block<MODE>(hd, hpA, hpB, cp, depthImg, colorImg, live, t, l, spec, bx, by, bz, ptr, fl, passed);
     }
     // U statistics: one 64-bit atomic per CTA
     passed = warp_sum_u(passed);
@@ -952,90 +974,6 @@ compactify_multi_kernel(BFHashDataStruct hd, const __grid_constant__ MultiFrusta
                 }
             }
         }
-    }
-}
-
-// truncation test of one voxel against one pose; returns true and the clamped sdf / colour when it passes (.cu:433-463)
-__device__ __forceinline__ bool probe_voxel(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depthImg,
-                                            const uchar4* __restrict__ colorImg, F3 world, float& sdfOut, uchar4& colOut) {
-    const F3 pf = xform(hp.m_rigidTransformInverse, world);
-    const float sx = pf.x * cp.fx / pf.z + cp.mx;
-    const float sy = pf.y * cp.fy / pf.z + cp.my;
-    unsigned px, py;
-    if (!(pixel_index(sx + 0.5f, cp.m_imageWidth, px) && pixel_index(sy + 0.5f, cp.m_imageHeight, py))) return false;
-    const float depth = __ldg(&depthImg[py * cp.m_imageWidth + px]);
-    if (!(depth != -INFINITY && depth < hp.m_maxIntegrationDistance)) return false;
-    float sdf = depth - pf.z;
-    const float trunc = truncation(hp, depth);
-    if (!(fabsf(sdf) < trunc)) return false;
-    sdfOut = (sdf >= 0.0f) ? fminf(trunc, sdf) : fmaxf(-trunc, sdf);
-    colOut = __ldg(&colorImg[py * cp.m_imageWidth + px]);
-    return true;
-}
-
-#define BF_REINT_MINBLOCKS 8
-__global__ void __launch_bounds__(128, BF_REINT_MINBLOCKS)
-reintegrate_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hpOld, const __grid_constant__ BFHashParams hpNew,
-                   const __grid_constant__ BFDepthCameraParams cp, const float* __restrict__ depthImg, const uchar4* __restrict__ colorImg,
-                   const int4* __restrict__ work, int set, unsigned* ctrs, int* __restrict__ live) {
-    const unsigned* countPtr = ctrs + set + SET_COUNT;
-    const unsigned count = ctrs[set + SET_WORK];
-    const unsigned t = threadIdx.x;
-    const int lx = (int)((4 * t) & 7), ly = (int)(((4 * t) & 63) >> 3), lz = (int)((4 * t) >> 6);
-    unsigned passed = 0;
-    const bool spec = count < BF_SPEC_BLOCKS;           // see integrate_kernel
-    int4 wNext = make_int4(0, 0, 0, 0);
-    if (blockIdx.x < count) wNext = __ldg(&work[blockIdx.x]);
-    for (unsigned b = blockIdx.x; b < count; b += gridDim.x) {
-        const int4 w = wNext;
-        if (b + gridDim.x < count) wNext = __ldg(&work[b + gridDim.x]);
-        const int bx = w.x, by = w.y, bz = w.z;
-        const unsigned ptr = ((unsigned)w.w & 0x0FFFFFFFu) * BF_SDF_BLOCK_VOXELS;
-        const unsigned fl = (unsigned)w.w >> 28;        // bit0: the old pose can touch this block, bit1: the new pose can
-        uint4* const vp = reinterpret_cast<uint4*>(hd.d_SDFBlocks + (size_t)ptr) + 3 * t;
-        VoxelQuad q;
-        if (spec) { q.a = vp[0]; q.b = vp[1]; q.c = vp[2]; }
-        float sdfD[4], sdfI[4];
-        uchar4 colD[4], colI[4];
-        unsigned maskD = 0, maskI = 0;
-        int liveDelta = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const I3 pi = { bx * BF_SDF_BLOCK_SIZE + lx + k, by * BF_SDF_BLOCK_SIZE + ly, bz * BF_SDF_BLOCK_SIZE + lz };
-            const F3 world = voxel_to_world(hpNew, pi);       // both poses of one scene share the voxel size (checked by the host)
-            if ((fl & 1u) && probe_voxel(hpOld, cp, depthImg, colorImg, world, sdfD[k], colD[k])) maskD |= 1u << k;
-            if ((fl & 2u) && probe_voxel(hpNew, cp, depthImg, colorImg, world, sdfI[k], colI[k])) maskI |= 1u << k;
-        }
-        const unsigned mask = maskD | maskI;
-        if (mask) {
-            if (!spec) { q.a = vp[0]; q.b = vp[1]; q.c = vp[2]; }
-            if (maskD & 1u) update_voxel<true>(hpOld, sdfD[0], colD[0], q.a.x, q.a.y, q.a.z, liveDelta);
-            if (maskI & 1u) update_voxel<false>(hpNew, sdfI[0], colI[0], q.a.x, q.a.y, q.a.z, liveDelta);
-            if (maskD & 2u) update_voxel<true>(hpOld, sdfD[1], colD[1], q.a.w, q.b.x, q.b.y, liveDelta);
-            if (maskI & 2u) update_voxel<false>(hpNew, sdfI[1], colI[1], q.a.w, q.b.x, q.b.y, liveDelta);
-            if (maskD & 4u) update_voxel<true>(hpOld, sdfD[2], colD[2], q.b.z, q.b.w, q.c.x, liveDelta);
-            if (maskI & 4u) update_voxel<false>(hpNew, sdfI[2], colI[2], q.b.z, q.b.w, q.c.x, liveDelta);
-            if (maskD & 8u) update_voxel<true>(hpOld, sdfD[3], colD[3], q.c.y, q.c.z, q.c.w, liveDelta);
-            if (maskI & 8u) update_voxel<false>(hpNew, sdfI[3], colI[3], q.c.y, q.c.z, q.c.w, liveDelta);
-            if (mask & 0x3u) vp[0] = q.a;
-            if (mask & 0x6u) vp[1] = q.b;
-            if (mask & 0xCu) vp[2] = q.c;
-            passed += __popc(maskD) + __popc(maskI);
-        }
-        if (__any_sync(0xffffffffu, liveDelta != 0)) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) liveDelta += __shfl_xor_sync(0xffffffffu, liveDelta, o);
-            if ((t & 31) == 0 && liveDelta != 0) atomicAdd(&live[ptr / BF_SDF_BLOCK_VOXELS], liveDelta);
-        }
-    }
-    passed = warp_sum_u(passed);
-    __shared__ unsigned sPassed[4];
-    if ((t & 31) == 0) sPassed[t >> 5] = passed;
-    __syncthreads();
-    if (t == 0) {
-        const unsigned long long tot = (unsigned long long)sPassed[0] + sPassed[1] + sPassed[2] + sPassed[3];
-        if (tot) { atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[set + SET_U_LO]), tot); atomicAdd(reinterpret_cast<unsigned long long*>(&ctrs[CTR_U_TOT_LO]), tot); }
-        if (blockIdx.x == 0) { const unsigned listCount = *countPtr; hd.d_hashCompactifiedCounter[0] = (int)listCount; ctrs[CTR_E] = listCount; }
     }
 }
 
@@ -1311,18 +1249,22 @@ static int do_alloc(BFHashDataStruct* hd, const BFHashParams* hp, const float* d
 }
 
 // useWork: also emit the stencil work list (library sequences).  setZeroed: the preceding launch (alloc_kernel) already zeroed
-// the counter set of the new parity.
-static int do_compactify(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, TsdfAux* aux, bool useWork, bool setZeroed) {
+// the counter set of the new parity.  hpOld (fused re-integration, useWork): the union list of hpOld's and hp's frusta, with the
+// per-pose bits in listFlags and in the work items.
+static int do_compactify(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, TsdfAux* aux, bool useWork, bool setZeroed,
+                         const BFHashParams* hpOld = nullptr) {
     aux->parity ^= 1u;
-    aux->lastListDual = false;
+    aux->lastListDual = hpOld != nullptr;
     const int set = set_of(aux->parity);
     if (!setZeroed) {
         int rc = front_acquire_set(aux, aux->parity); if (rc) return rc;
         BF_CHECK(cudaMemsetAsync(aux->ctrs + set, 0, SET_WORDS * sizeof(unsigned), g_stream));
     }
     ++g_launchCount;
-    compactify_kernel<<<grid_for((hp->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(*hd, *hp, *cp, aux->slotInfo, aux->ctrs, set,
-                                                                                            useWork ? aux->work2[aux->parity] : nullptr);
+    const int grid = grid_for((hp->m_numSDFBlocks + 255) / 256, 4);
+    int4* const work = useWork ? aux->work2[aux->parity] : nullptr;
+    if (hpOld) compactify_dual_kernel<<<grid, 256, 0, g_stream>>>(*hd, *hpOld, *hp, *cp, aux->slotInfo, aux->ctrs, set, aux->listFlags, work);
+    else       compactify_kernel<<<grid, 256, 0, g_stream>>>(*hd, *hp, *cp, aux->slotInfo, aux->ctrs, set, work);
     BF_CHECK(cudaGetLastError());
     if (aux->pipeOpen) BF_CHECK(cudaEventRecord(aux->evList[aux->parity], g_stream));
     return 0;
@@ -1339,38 +1281,68 @@ static int stencil_end(TsdfAux* aux) {
     if (aux->pipeOpen) { BF_CHECK(cudaEventRecord(aux->evStencil[aux->parity], aux->lane)); aux->stencilPending[aux->parity] = true; }
     return 0;
 }
+
+// The bookkeeping around one stencil launch on stream s: the launch count, the profile counters and, while profiling, a pair of CUDA
+// events -- for a batch launch also the in-kernel %globaltimer bracket, whose slot launch(ktime) receives (nullptr otherwise).
+// frames: the frame images the launch reads.
+template <class Launch>
+static int profiled_launch(cudaStream_t s, bool batch, unsigned frames, Launch launch) {
+    const bool timeIt = g_prof.on && g_prof.used < kMaxProfiledLaunches;
+    if (g_prof.on) {
+        ++g_prof.launches; g_prof.frames += frames;
+        if (batch) { ++g_prof.batchLaunches; g_prof.batchFrames += frames; }
+    }
+    unsigned long long* ktime = nullptr;
+    if (timeIt) {
+        if (g_prof.ev.size() <= g_prof.used) {
+            TimedLaunch e{};
+            BF_CHECK(cudaEventCreate(&e.start)); BF_CHECK(cudaEventCreate(&e.stop));
+            g_prof.ev.push_back(e);
+        }
+        g_prof.ev[g_prof.used].batch = batch;
+        if (batch) {
+            if (!g_prof.ktime) BF_CHECK(cudaMalloc(&g_prof.ktime, sizeof(unsigned long long) * 2 * kMaxProfiledLaunches));
+            ktime = g_prof.ktime + 2 * g_prof.used;
+            BF_CHECK(cudaMemsetAsync(ktime, 0xff, sizeof(unsigned long long), s));
+            BF_CHECK(cudaMemsetAsync(ktime + 1, 0, sizeof(unsigned long long), s));
+        }
+        BF_CHECK(cudaEventRecord(g_prof.ev[g_prof.used].start, s));
+    }
+    ++g_launchCount;
+    const int rc = launch(ktime);
+    if (rc) return rc;
+    BF_CHECK(cudaGetLastError());
+    if (timeIt) { BF_CHECK(cudaEventRecord(g_prof.ev[g_prof.used].stop, s)); ++g_prof.used; }
+    return 0;
+}
+
 // CTAs per SM of the exact stencils, inside a two-lane bracket too.  Capping the stencil at 4-6 CTAs per SM so that alloc CTAs can
 // co-reside slows the stencil by more than the overlap returns; uncapped, the front lane fills the SMs the stencil's last wave frees.
 static const int kStencilCtasPerSm = 16;
 
-static int do_integrate(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraData* dd, const BFDepthCameraParams* cp,
-                        TsdfAux* aux, bool deIntegrate, bool useListCount, unsigned countOverride) {
-    const unsigned upper = useListCount ? hp->m_numSDFBlocks : countOverride;
+// One stencil over the live list, on the back lane, in the selected arithmetic.  mode as integrate_kernel's MODE: 0 integrate / 1 de-integrate
+// with hpA (hpB = hpA), 2 the fused re-integration pair (hpA the old pose, hpB the new one).  useListCount / countOverride as integrate_kernel's;
+// the stubs' list (countOverride) has no work list.
+static int do_stencil(BFHashDataStruct* hd, const BFHashParams* hpA, const BFHashParams* hpB, const BFDepthCameraData* dd, const BFDepthCameraParams* cp,
+                      TsdfAux* aux, int mode, bool useListCount, unsigned countOverride) {
+    const unsigned upper = useListCount ? hpB->m_numSDFBlocks : countOverride;
     if (upper == 0) return 0;
-    const uchar4* color = reinterpret_cast<const uchar4*>(dd->d_colorData);
     const cudaStream_t sb = back_lane(aux);
     int rc = stencil_begin(aux); if (rc) return rc;
-    const bool timeIt = g_profile && g_evUsed < kMaxProfiledLaunches;
-    if (g_profile) { ++g_profLaunches; ++g_profFrames; }
-    if (timeIt) {
-        if (g_evStart.size() <= g_evUsed) { cudaEvent_t a, b; BF_CHECK(cudaEventCreate(&a)); BF_CHECK(cudaEventCreate(&b)); g_evStart.push_back(a); g_evStop.push_back(b); }
-        if (g_evIsBatch.size() > g_evUsed) g_evIsBatch[g_evUsed] = 0;
-        BF_CHECK(cudaEventRecord(g_evStart[g_evUsed], sb));
-    }
-    ++g_launchCount;
     const int set = set_of(aux->parity);
-    const int4* work = useListCount ? aux->work2[aux->parity] : nullptr;        // the stubs' list (countOverride) has no work list
-    if (arith_fast()) {
-        rc = launch_integrate_fast(hd, hp, cp, dd->d_depthData, dd->d_colorData, deIntegrate, useListCount, countOverride, aux->ctrs, aux->live, work, set,
-                                   grid_for(upper, fast_stencil_ctas_per_sm(false)), sb);
-        if (rc) return rc;
-    } else {
-        const int grid = grid_for(upper, kStencilCtasPerSm);
-        if (deIntegrate) integrate_kernel<true><<<grid, 128, 0, sb>>>(*hd, *hp, *cp, dd->d_depthData, color, useListCount ? 1 : 0, countOverride, aux->ctrs, aux->live, work, set);
-        else             integrate_kernel<false><<<grid, 128, 0, sb>>>(*hd, *hp, *cp, dd->d_depthData, color, useListCount ? 1 : 0, countOverride, aux->ctrs, aux->live, work, set);
-    }
-    BF_CHECK(cudaGetLastError());
-    if (timeIt) { BF_CHECK(cudaEventRecord(g_evStop[g_evUsed], sb)); ++g_evUsed; }
+    const int4* work = useListCount ? aux->work2[aux->parity] : nullptr;
+    rc = profiled_launch(sb, false, 1, [&](unsigned long long*) {
+        if (arith_fast()) {
+            const int grid = grid_for(upper, fast_stencil_ctas_per_sm(mode == 2));
+            if (mode == 2) return launch_reintegrate_fast(hd, hpA, hpB, cp, dd->d_depthData, dd->d_colorData, work, set, aux->ctrs, aux->live, grid, sb);
+            return launch_integrate_fast(hd, hpA, cp, dd->d_depthData, dd->d_colorData, mode == 1, useListCount, countOverride, aux->ctrs, aux->live, work, set, grid, sb);
+        }
+        auto* const kernel = mode == 0 ? integrate_kernel<0> : (mode == 1 ? integrate_kernel<1> : integrate_kernel<2>);
+        kernel<<<grid_for(upper, kStencilCtasPerSm), 128, 0, sb>>>(*hd, *hpA, *hpB, *cp, dd->d_depthData, reinterpret_cast<const uchar4*>(dd->d_colorData),
+                                                                 useListCount ? 1 : 0, countOverride, aux->ctrs, aux->live, work, set);
+        return 0;
+    });
+    if (rc) return rc;
     return stencil_end(aux);
 }
 
@@ -1433,7 +1405,7 @@ BF_API int bfTsdfIntegrateFrame(BFHashDataStruct* hd, const BFHashParams* hp, co
     if (rc) return rc;
     if (!deIntegrate) { rc = do_alloc(hd, hp, dd->d_depthData, cp, aux, (int)(aux->parity ^ 1u)); if (rc) return rc; }
     rc = do_compactify(hd, hp, cp, aux, true, /*setZeroed=*/!deIntegrate); if (rc) return rc;
-    return do_integrate(hd, hp, dd, cp, aux, deIntegrate != 0, true, 0);
+    return do_stencil(hd, hp, hp, dd, cp, aux, deIntegrate ? 1 : 0, true, 0);
 }
 
 // CUDASceneRepHashSDF::deIntegrate(old pose) immediately followed by ::integrate(new pose) of the SAME frame
@@ -1446,35 +1418,8 @@ BF_API int bfTsdfReintegrateFrame(BFHashDataStruct* hd, const BFHashParams* hpOl
     if (dd->d_colorData == nullptr) return do_alloc(hd, hpNew, dd->d_depthData, cp, aux, -1);     // no colour: neither pass updates a voxel
     if (aux->work == nullptr || hpOld->m_virtualVoxelSize != hpNew->m_virtualVoxelSize) return (int)cudaErrorNotSupported;
     rc = do_alloc(hd, hpNew, dd->d_depthData, cp, aux, (int)(aux->parity ^ 1u)); if (rc) return rc;
-    aux->parity ^= 1u;
-    aux->lastListDual = true;
-    const int set = set_of(aux->parity);
-    ++g_launchCount;
-    compactify_dual_kernel<<<grid_for((hpNew->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(*hd, *hpOld, *hpNew, *cp, aux->slotInfo, aux->ctrs, set, aux->listFlags,
-                                                                                                    aux->work2[aux->parity]);
-    BF_CHECK(cudaGetLastError());
-    if (aux->pipeOpen) BF_CHECK(cudaEventRecord(aux->evList[aux->parity], g_stream));
-    const cudaStream_t sb = back_lane(aux);
-    rc = stencil_begin(aux); if (rc) return rc;
-    const bool timeIt = g_profile && g_evUsed < kMaxProfiledLaunches;
-    if (g_profile) { ++g_profLaunches; ++g_profFrames; }
-    if (timeIt) {
-        if (g_evStart.size() <= g_evUsed) { cudaEvent_t a, b; BF_CHECK(cudaEventCreate(&a)); BF_CHECK(cudaEventCreate(&b)); g_evStart.push_back(a); g_evStop.push_back(b); }
-        if (g_evIsBatch.size() > g_evUsed) g_evIsBatch[g_evUsed] = 0;
-        BF_CHECK(cudaEventRecord(g_evStart[g_evUsed], sb));
-    }
-    ++g_launchCount;
-    if (arith_fast()) {
-        rc = launch_reintegrate_fast(hd, hpOld, hpNew, cp, dd->d_depthData, dd->d_colorData, aux->work2[aux->parity], set, aux->ctrs, aux->live,
-                                     grid_for(hpNew->m_numSDFBlocks, fast_stencil_ctas_per_sm(true)), sb);
-        if (rc) return rc;
-    } else {
-        reintegrate_kernel<<<grid_for(hpNew->m_numSDFBlocks, kStencilCtasPerSm), 128, 0, sb>>>(
-            *hd, *hpOld, *hpNew, *cp, dd->d_depthData, reinterpret_cast<const uchar4*>(dd->d_colorData), aux->work2[aux->parity], set, aux->ctrs, aux->live);
-    }
-    BF_CHECK(cudaGetLastError());
-    if (timeIt) { BF_CHECK(cudaEventRecord(g_evStop[g_evUsed], sb)); ++g_evUsed; }
-    return stencil_end(aux);
+    rc = do_compactify(hd, hpNew, cp, aux, true, /*setZeroed=*/true, hpOld); if (rc) return rc;
+    return do_stencil(hd, hpOld, hpNew, dd, cp, aux, 2, true, 0);
 }
 
 // Up to BF_MULTI_MAX_OPS re-integration pairs {deIntegrate(frame f, old pose); integrate(frame f, new pose)} -- the loop body of
@@ -1540,22 +1485,11 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
                                                                                                  aux->listFlags, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots,
                                                                                                  aux->tilesMulti);
     BF_CHECK(cudaGetLastError());
-    const bool timeIt = g_profile && g_evUsed < kMaxProfiledLaunches;
-    if (g_profile) { ++g_profLaunches; g_profFrames += (unsigned long long)numPairs; ++g_profBatchLaunches; g_profBatchFrames += (unsigned long long)numPairs; }
-    if (timeIt) {
-        if (g_evStart.size() <= g_evUsed) { cudaEvent_t a, b; BF_CHECK(cudaEventCreate(&a)); BF_CHECK(cudaEventCreate(&b)); g_evStart.push_back(a); g_evStop.push_back(b); }
-        if (g_evIsBatch.size() <= g_evUsed) g_evIsBatch.resize(g_evUsed + 1, 0);
-        g_evIsBatch[g_evUsed] = 1;
-        if (!g_ktime) BF_CHECK(cudaMalloc(&g_ktime, sizeof(unsigned long long) * 2 * kMaxProfiledLaunches));
-        BF_CHECK(cudaMemsetAsync(g_ktime + 2 * g_evUsed, 0xff, sizeof(unsigned long long), g_stream));
-        BF_CHECK(cudaMemsetAsync(g_ktime + 2 * g_evUsed + 1, 0, sizeof(unsigned long long), g_stream));
-        BF_CHECK(cudaEventRecord(g_evStart[g_evUsed], g_stream));
-    }
-    ++g_launchCount;
-    rc = launch_reintegrate_multi_fast(hd, desc, numPairs, cp, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots, set, aux->ctrs, aux->live,
-                                       grid_for(hp->m_numSDFBlocks, fast_stencil_ctas_per_sm(true)), g_stream, timeIt ? g_ktime + 2 * g_evUsed : nullptr);
+    rc = profiled_launch(g_stream, true, (unsigned)numPairs, [&](unsigned long long* ktime) {
+        return launch_reintegrate_multi_fast(hd, desc, numPairs, cp, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots, set,
+                                             aux->ctrs, aux->live, grid_for(hp->m_numSDFBlocks, fast_stencil_ctas_per_sm(true)), g_stream, ktime);
+    });
     if (rc) return rc;
-    if (timeIt) { BF_CHECK(cudaEventRecord(g_evStop[g_evUsed], g_stream)); ++g_evUsed; }
     *hp = hpNew[numPairs - 1];
     return 0;
 }
@@ -1606,16 +1540,19 @@ BF_API int bfTsdfGetLastFrameStats(const BFHashDataStruct* hd, unsigned long lon
 
 BF_API unsigned long long bfGetLaunchCount(void) { return g_launchCount; }
 
+// restart the running U / E sums of one table's counters
+static int restart_sums(unsigned* ctrs) {
+    BF_CHECK(cudaMemsetAsync(ctrs + CTR_U_TOT_LO, 0, 4 * sizeof(unsigned), g_stream));
+    BF_CHECK(cudaMemsetAsync(ctrs + CTR_UB_TOT_LO, 0, 4 * sizeof(unsigned), g_stream));
+    BF_CHECK(cudaMemsetAsync(ctrs + CTR_CULLB, 0, sizeof(unsigned), g_stream));
+    return 0;
+}
+
 BF_API int bfTsdfSetProfiling(int enable) {
-    g_profile = enable != 0;
-    g_evUsed = 0; g_profLaunches = 0; g_profFrames = 0; g_profBatchLaunches = 0; g_profBatchFrames = 0;
-    std::fill(g_evIsBatch.begin(), g_evIsBatch.end(), 0);
+    g_prof.on = enable != 0;
+    g_prof.reset();
     std::lock_guard<std::mutex> lk(g_auxMutex);
-    for (auto& kv : g_aux) {                    // restart the U / E sums
-        BF_CHECK(cudaMemsetAsync(kv.second.ctrs + CTR_U_TOT_LO, 0, 4 * sizeof(unsigned), g_stream));
-        BF_CHECK(cudaMemsetAsync(kv.second.ctrs + CTR_UB_TOT_LO, 0, 4 * sizeof(unsigned), g_stream));
-        BF_CHECK(cudaMemsetAsync(kv.second.ctrs + CTR_CULLB, 0, sizeof(unsigned), g_stream));
-    }
+    for (auto& kv : g_aux) { const int rc = restart_sums(kv.second.ctrs); if (rc) return rc; }
     return 0;
 }
 
@@ -1629,35 +1566,32 @@ BF_API int bfTsdfGetProfileEx(const BFHashDataStruct* hd, unsigned long long out
     if (rc) return rc;
     BF_CHECK(cudaStreamSynchronize(g_stream));
     double ms = 0.0, msB = 0.0; unsigned long long nB = 0;
-    for (size_t i = 0; i < g_evUsed; ++i) {
-        float t = 0.0f; BF_CHECK(cudaEventElapsedTime(&t, g_evStart[i], g_evStop[i])); ms += t;
-        if (i < g_evIsBatch.size() && g_evIsBatch[i]) { msB += t; ++nB; }
+    for (size_t i = 0; i < g_prof.used; ++i) {
+        float t = 0.0f; BF_CHECK(cudaEventElapsedTime(&t, g_prof.ev[i].start, g_prof.ev[i].stop)); ms += t;
+        if (g_prof.ev[i].batch) { msB += t; ++nB; }
     }
     unsigned c[CTR_NUM];
     BF_CHECK(cudaMemcpy(c, aux->ctrs, sizeof(c), cudaMemcpyDeviceToHost));
     for (int k = 0; k < 16; ++k) out[k] = 0;
-    out[0] = g_profLaunches; out[1] = g_evUsed; out[2] = (unsigned long long)(ms * 1e6);
+    out[0] = g_prof.launches; out[1] = g_prof.used; out[2] = (unsigned long long)(ms * 1e6);
     out[3] = ((unsigned long long)c[CTR_U_TOT_HI] << 32) | c[CTR_U_TOT_LO];
     out[4] = ((unsigned long long)c[CTR_E_TOT_HI] << 32) | c[CTR_E_TOT_LO];
-    out[5] = g_profFrames;          // frame images read by those launches (a batch launch reads one per re-integration pair)
-    out[8] = g_profBatchLaunches; out[9] = nB; out[10] = (unsigned long long)(msB * 1e6);
+    out[5] = g_prof.frames;         // frame images read by those launches (a batch launch reads one per re-integration pair)
+    out[8] = g_prof.batchLaunches; out[9] = nB; out[10] = (unsigned long long)(msB * 1e6);
     out[11] = ((unsigned long long)c[CTR_UB_TOT_HI] << 32) | c[CTR_UB_TOT_LO];
     out[12] = ((unsigned long long)c[CTR_EB_TOT_HI] << 32) | c[CTR_EB_TOT_LO];
-    out[13] = g_profBatchFrames;
+    out[13] = g_prof.batchFrames;
     out[15] = c[CTR_CULLB];         // (block, op, pose) probes the batch cull removed (E counts them: they are in-frustum)
-    if (g_ktime && g_evUsed) {          // out[14]: the batch launches' duration by the in-kernel %globaltimer brackets (first CTA start -> last CTA end), ns
-        std::vector<unsigned long long> kt(2 * g_evUsed);
-        BF_CHECK(cudaMemcpy(kt.data(), g_ktime, sizeof(unsigned long long) * 2 * g_evUsed, cudaMemcpyDeviceToHost));
+    if (g_prof.ktime && g_prof.used) {  // out[14]: the batch launches' duration by the in-kernel %globaltimer brackets (first CTA start -> last CTA end), ns
+        std::vector<unsigned long long> kt(2 * g_prof.used);
+        BF_CHECK(cudaMemcpy(kt.data(), g_prof.ktime, sizeof(unsigned long long) * 2 * g_prof.used, cudaMemcpyDeviceToHost));
         unsigned long long sum = 0;
-        for (size_t i = 0; i < g_evUsed; ++i) if (i < g_evIsBatch.size() && g_evIsBatch[i] && kt[2 * i + 1] > kt[2 * i]) sum += kt[2 * i + 1] - kt[2 * i];
+        for (size_t i = 0; i < g_prof.used; ++i) if (g_prof.ev[i].batch && kt[2 * i + 1] > kt[2 * i]) sum += kt[2 * i + 1] - kt[2 * i];
         out[14] = sum;
     }
     // restart accumulation
-    BF_CHECK(cudaMemsetAsync(aux->ctrs + CTR_U_TOT_LO, 0, 4 * sizeof(unsigned), g_stream));
-    BF_CHECK(cudaMemsetAsync(aux->ctrs + CTR_UB_TOT_LO, 0, 4 * sizeof(unsigned), g_stream));
-    BF_CHECK(cudaMemsetAsync(aux->ctrs + CTR_CULLB, 0, sizeof(unsigned), g_stream));
-    g_evUsed = 0; g_profLaunches = 0; g_profFrames = 0; g_profBatchLaunches = 0; g_profBatchFrames = 0;
-    std::fill(g_evIsBatch.begin(), g_evIsBatch.end(), 0);
+    rc = restart_sums(aux->ctrs); if (rc) return rc;
+    g_prof.reset();
     return 0;
 }
 BF_API int bfTsdfGetProfile(const BFHashDataStruct* hd, unsigned long long out[8]) {
@@ -1731,7 +1665,7 @@ BF_API unsigned int compactifyHashAllInOneCUDA(BFHashDataStruct* hd, const BFHas
 static void integrate_stub(BFHashDataStruct* hd, const BFHashParams* hp, bool de) {
     TsdfAux* aux;
     BF_SAFE(get_aux(hd, &g_hashParams, &aux, true));
-    BF_SAFE(do_integrate(hd, &g_hashParams, &g_bound, &g_camParams, aux, de, false, hp->m_numOccupiedBlocks));
+    BF_SAFE(do_stencil(hd, &g_hashParams, &g_hashParams, &g_bound, &g_camParams, aux, de ? 1 : 0, false, hp->m_numOccupiedBlocks));
 }
 BF_API void integrateDepthMapCUDA(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraData*, const BFDepthCameraParams*) { integrate_stub(hd, hp, false); }
 BF_API void deIntegrateDepthMapCUDA(BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraData*, const BFDepthCameraParams*) { integrate_stub(hd, hp, true); }

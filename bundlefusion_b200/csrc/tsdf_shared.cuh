@@ -15,7 +15,7 @@ enum { CTR_HIGH_WATER = 0, CTR_E = 3, CTR_UB_TOT_LO = 4, CTR_UB_TOT_HI = 5, CTR_
        SET_COUNT = 0, SET_WORK = 1, SET_Q2 = 2, SET_TICKET = 3 /* dynamic block deal of the fast stencil */, SET_U_LO = 4, SET_U_HI = 5, SET_Q1 = 6, SET_Q0 = 7 /* batch: items of cost quartile 2 / 1 / 0 (quartile 3: SET_WORK) */, SET_WORDS = 8 };
 
 // tolerance-mode stencils (tsdf_fast.cu).  `work` may be NULL (the list is then d_hashCompactified[0..count)); useListCount /
-// countOverride as in tsdf.cu's integrate_kernel.
+// countOverride as in tsdf.cu's integrate_kernel<MODE>.
 int launch_integrate_fast(const BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, const float* depth, const void* color,
                           bool deIntegrate, bool useListCount, unsigned countOverride, unsigned* ctrs, int* live, const int4* work, int set,
                           int grid, cudaStream_t s);
