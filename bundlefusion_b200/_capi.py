@@ -158,7 +158,7 @@ BUNDLER_SYMBOLS = ["computeSiftTransformCU", "initNextGlobalTransformCU", "updat
 SIFT_SYMBOLS = ["bfSiftMatchBatch", "bfSiftSortKeyPointMatches", "bfSiftFilterKeyPointMatches", "bfSiftFilterMatchesBySurfaceArea", "bfSiftFilterMatchesByDenseVerify",
                 "bfSiftAddCurrToResiduals", "bfSiftWorkspaceBytes", "bfSiftReleaseWorkspace", "bfSiftReserveWorkspace", "bfSiftDetect", "bfSiftDetectWorkspaceBytes",
                 "bfSiftDetectReleaseWorkspace", "bfSiftInvalidateImageToImage", "bfSiftCheckForInvalidFrames", "bfSiftFilterFrames",
-                "bfSiftAddCurrToResidualsIfMatched", "bfSiftVerifyTrajectory", "bfSiftFuseToGlobal"]
+                "bfSiftAddCurrToResidualsIfMatched", "bfSiftVerifyTrajectory", "bfSiftFuseToGlobal", "bfSiftSetMatchSweep", "bfSiftGetMatchInfo"]
 
 SOLVER_SYMBOLS = [
     "solveBundlingStub", "buildVariablesToCorrespondencesTableCUDA", "evalMaxResidual", "countHighResiduals", "collectHighResiduals",
@@ -357,6 +357,9 @@ def lib() -> C.CDLL:
     L.bfTrajectorySelectReintegration.argtypes = [vp, vp, vp, C.c_uint, C.c_uint, C.c_float, C.c_float, vp, vp, vp]
     # SIFT descriptor matcher
     L.bfSiftMatchBatch.argtypes = [P(BFSiftMatchJob), C.c_int, C.c_float, C.c_float]
+    L.bfSiftSetMatchSweep.argtypes = [C.c_int]
+    L.bfSiftSetMatchSweep.restype = C.c_int
+    L.bfSiftGetMatchInfo.argtypes = [C.c_int * 2]
     L.bfSiftSortKeyPointMatches.argtypes = [C.c_uint, C.c_uint, C.c_uint, vp, vp, vp]
     L.bfSiftFilterKeyPointMatches.argtypes = [C.c_uint, C.c_uint, C.c_uint] + [vp] * 9 + [P(C.c_float), C.c_uint, C.c_float]
     L.bfSiftAddCurrToResiduals.argtypes = [C.c_uint, C.c_uint, C.c_uint] + [vp] * 6 + [P(C.c_float)]

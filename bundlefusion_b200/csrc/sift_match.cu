@@ -14,6 +14,8 @@
 //  * all pairs of a frame are ONE batch: two launches in total instead of (2 copies + 3 launches + 1 memset) per pair.
 #include <cuda.h>
 
+#include <atomic>
+#include <cstring>
 #include <map>
 #include <mutex>
 #include <vector>
@@ -449,9 +451,19 @@ struct SiftWs {
     int* colResult = nullptr; size_t colCap = 0;
     int* done = nullptr;
     CUtensorMap* dMaps = nullptr; CUtensorMap* hMaps = nullptr; size_t mapCap = 0;      // two tensor maps per job (device table + pinned staging)
+    std::vector<CUtensorMap> mapStage;                                                  // a batch's maps, encoded before anything is enqueued
     std::map<std::pair<const void*, int>, CUtensorMap> mapCache;                        // encoded maps by (array, rows): a keyframe's descriptors recur every frame
 };
 static SiftWs g_sift;
+// Which sweep runs a batch (bfSiftSetMatchSweep): auto = wgmma + TMA unless the batch's arrays cannot be described by tensor maps (no driver
+// entry point), then mma.sync.  The setting starts as BF_SIFT_MATCH gives it ("mma": the mma.sync sweep).  A forced sweep never falls back, so
+// that a test can run one batch under both and compare the bytes.
+static std::atomic<int>& sweep_setting() {
+    static std::atomic<int> s{ [] { const char* e = getenv("BF_SIFT_MATCH"); return (e && e[0] == 'm') ? BF_SIFT_SWEEP_MMA : BF_SIFT_SWEEP_AUTO; }() };
+    return s;
+}
+static bool g_wgmmaAttrSet = false;                // the wgmma kernels' dynamic shared memory limit has been raised (at their first use)
+static int g_matchInfo[2] = { 0, 0 };              // the last batch: sweep that ran, jobs (bfSiftGetMatchInfo)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static EncodeTiledFn encode_tiled_fn() {
@@ -528,26 +540,44 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
     size_t rows = 0, cols = 0;
     int maxN1 = 0, maxN2 = 0;
     for (int i = 0; i < numJobs; ++i) {
-        if (jobs[i].num1 > 0 && jobs[i].num2 > 0) { rows += (size_t)jobs[i].num1; cols += (size_t)jobs[i].num2; maxN1 = jobs[i].num1 > maxN1 ? jobs[i].num1 : maxN1; maxN2 = jobs[i].num2 > maxN2 ? jobs[i].num2 : maxN2; }
+        const bool live = jobs[i].num1 > 0 && jobs[i].num2 > 0;
+        if (live) { rows += (size_t)jobs[i].num1; cols += (size_t)jobs[i].num2; maxN1 = jobs[i].num1 > maxN1 ? jobs[i].num1 : maxN1; maxN2 = jobs[i].num2 > maxN2 ? jobs[i].num2 : maxN2; }
         if (jobs[i].num1 >= (1 << 24) || jobs[i].num2 >= (1 << 24)) return (int)cudaErrorInvalidValue;       // index field of the packed key
+        // both sweeps read descriptor rows in 16-byte units (TMA boxes, uint4 loads): a misaligned array is refused before anything is enqueued
+        if (live && ((reinterpret_cast<uintptr_t>(jobs[i].d_des1) | reinterpret_cast<uintptr_t>(jobs[i].d_des2)) & 15u)) {
+            set_last_error("bfSiftMatchBatch: descriptor array not 16-byte aligned", cudaErrorInvalidValue);
+            return (int)cudaErrorInvalidValue;
+        }
+    }
+    // tensor maps of the batch (wgmma + TMA sweep), encoded on the host before anything is enqueued: a forced wgmma sweep that cannot map a batch
+    // fails it here; auto runs such a batch (no driver entry point) with the mma.sync sweep, which computes the same matches
+    const int sweep = sweep_setting().load();
+    bool useTc = sweep != BF_SIFT_SWEEP_MMA;
+    if (useTc) {
+        g_sift.mapStage.resize(2 * (size_t)numJobs);
+        for (int i = 0; i < numJobs && useTc; ++i) {
+            const BFSiftMatchJob& j = jobs[i];
+            if (j.num1 > 0 && j.num2 > 0)
+                useTc = descriptor_map(j.d_des1, j.num1, &g_sift.mapStage[2 * (size_t)i]) && descriptor_map(j.d_des2, j.num2, &g_sift.mapStage[2 * (size_t)i + 1]);
+        }
+        if (!useTc && sweep == BF_SIFT_SWEEP_WGMMA) {
+            set_last_error("bfSiftMatchBatch: the forced wgmma sweep cannot map this batch", cudaErrorNotSupported);
+            return (int)cudaErrorNotSupported;
+        }
+    }
+    if (useTc && !g_wgmmaAttrSet) {
+        BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
+        BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
+        g_wgmmaAttrSet = true;
     }
     cudaStream_t s = stream();
     if (!g_sift.evDone) BF_CHECK(cudaEventCreateWithFlags(&g_sift.evDone, cudaEventDisableTiming));
     BF_CHECK(cudaStreamWaitEvent(s, g_sift.evDone, 0));       // a previous batch (possibly on another stream) still owns rowResult / the job table
     { const int rcR = sift_reserve(s, (size_t)numJobs, rows, cols, true); if (rcR) return rcR; }
-    // BF_SIFT_MATCH: "mma" = warp-level mma.sync sweep, default = wgmma + TMA.  A batch whose arrays cannot be described by tensor maps (base not
-    // 16-byte aligned, or no driver entry point) runs the mma.sync sweep, which computes the same matches.
-    static int path = -1;
-    if (path < 0) {
-        const char* e = getenv("BF_SIFT_MATCH");
-        path = (e && e[0] == 'm') ? 0 : 2;
-        if (path == 2) {
-            BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
-            BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
-        }
+    if (useTc) {
+        const int rcM = sift_reserve_maps(s, (size_t)numJobs, true); if (rcM) return rcM;
+        memcpy(g_sift.hMaps, g_sift.mapStage.data(), sizeof(CUtensorMap) * 2 * (size_t)numJobs);      // staging is free: sift_reserve waited for evCopied
     }
-    bool mapsOk = (path == 2);
-    if (mapsOk) { const int rcM = sift_reserve_maps(s, (size_t)numJobs, true); if (rcM) return rcM; }
     SiftJobDev* h = g_sift.hJobs;
     size_t off = 0, coff = 0;
     for (int i = 0; i < numJobs; ++i) {
@@ -560,20 +590,18 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
         r.offset = make_uint2(j.keyPointOffset[0], j.keyPointOffset[1]);
         r.colResult = g_sift.colResult + coff; r.done = g_sift.done + i;
         r.mapA = nullptr; r.mapB = nullptr;
-        if (mapsOk && live) {
-            if (descriptor_map(j.d_des1, j.num1, &g_sift.hMaps[2 * i]) && descriptor_map(j.d_des2, j.num2, &g_sift.hMaps[2 * i + 1])) { r.mapA = g_sift.dMaps + 2 * i; r.mapB = g_sift.dMaps + 2 * i + 1; }
-            else mapsOk = false;
-        }
+        if (useTc && live) { r.mapA = g_sift.dMaps + 2 * i; r.mapB = g_sift.dMaps + 2 * i + 1; }
         SiftJobDev c = r;                                   // column pass: image 2 owns the sweep, image 1 is swept
         c.desA = j.d_des2; c.nA = r.nB; c.desB = j.d_des1; c.nB = r.nA; c.mapA = r.mapB; c.mapB = r.mapA;
         h[i] = r; h[(size_t)numJobs + i] = c;
         if (live) { off += (size_t)j.num1; coff += (size_t)j.num2; }
     }
-    if (mapsOk) BF_CHECK(cudaMemcpyAsync(g_sift.dMaps, g_sift.hMaps, sizeof(CUtensorMap) * 2 * (size_t)numJobs, cudaMemcpyHostToDevice, s));
+    if (useTc) BF_CHECK(cudaMemcpyAsync(g_sift.dMaps, g_sift.hMaps, sizeof(CUtensorMap) * 2 * (size_t)numJobs, cudaMemcpyHostToDevice, s));
     BF_CHECK(cudaMemcpyAsync(g_sift.dJobs, h, sizeof(SiftJobDev) * 2 * (size_t)numJobs, cudaMemcpyHostToDevice, s));
     BF_CHECK(cudaEventRecord(g_sift.evCopied, s));
     g_launchCount += 2;
-    if (path == 2 && mapsOk) {
+    g_matchInfo[0] = useTc ? BF_SIFT_SWEEP_WGMMA : BF_SIFT_SWEEP_MMA; g_matchInfo[1] = numJobs;
+    if (useTc) {
         const int gx1 = maxN1 > 0 ? (maxN1 + TC_BM - 1) / TC_BM : 1, gx2 = maxN2 > 0 ? (maxN2 + TC_BM - 1) / TC_BM : 1;
         sift_best_wgmma_kernel<false><<<dim3(gx1, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs, distmax, ratiomax);
         BF_CHECK(cudaGetLastError());
@@ -623,5 +651,15 @@ BF_API int bfSiftReleaseWorkspace(void) {
     if (g_sift.evCopied) cudaEventDestroy(g_sift.evCopied);
     if (g_sift.evDone) cudaEventDestroy(g_sift.evDone);
     g_sift = SiftWs();
+    return 0;
+}
+BF_API int bfSiftSetMatchSweep(int sweep) {
+    if (sweep < BF_SIFT_SWEEP_AUTO || sweep > BF_SIFT_SWEEP_MMA) return (int)cudaErrorInvalidValue;
+    return sweep_setting().exchange(sweep);
+}
+BF_API int bfSiftGetMatchInfo(int out[2]) {
+    if (!out) return (int)cudaErrorInvalidValue;
+    std::lock_guard<std::mutex> lk(g_siftMutex);
+    out[0] = g_matchInfo[0]; out[1] = g_matchInfo[1];
     return 0;
 }

@@ -10,6 +10,25 @@ from ._capi import BFSiftMatchJob
 
 MAX_MATCHES_PER_IMAGE_PAIR_RAW = 128      # FL/GlobalDefines.h:8
 
+# Descriptor-match sweeps (include/bf_sift.h: bfSiftSetMatchSweep).  Both give the same bytes; AUTO runs wgmma + TMA where tensor maps can be encoded.
+SIFT_SWEEP_AUTO, SIFT_SWEEP_WGMMA, SIFT_SWEEP_MMA = 0, 1, 2
+
+
+def set_match_sweep(sweep: int) -> int:
+    """Force the sweep of every later bfSiftMatchBatch in this process (SIFT_SWEEP_AUTO restores the default).  Returns the previous
+    setting.  A forced wgmma sweep that cannot map a batch makes that batch fail; it never falls back."""
+    rc = capi.lib().bfSiftSetMatchSweep(int(sweep))
+    if sweep not in (SIFT_SWEEP_AUTO, SIFT_SWEEP_WGMMA, SIFT_SWEEP_MMA):
+        capi.check(rc, "bfSiftSetMatchSweep")
+    return rc
+
+
+def match_info() -> tuple[int, int]:
+    """(sweep that ran, number of jobs) of the last bfSiftMatchBatch that enqueued work; recorded on the host."""
+    out = (C.c_int * 2)()
+    capi.check(capi.lib().bfSiftGetMatchInfo(out), "bfSiftGetMatchInfo")
+    return out[0], out[1]
+
 
 class ImagePairMatch:
     """FL/SiftGPU/SIFTImageManager.h:38-42 -- device buffers of one image pair's raw matches."""
@@ -44,7 +63,8 @@ class SiftMatchGPU:
         self.lib.bfSetStream(C.c_void_p(t.cuda.current_stream(self.device).cuda_stream))
 
     def SetDescriptors(self, index: int, num: int, d_descriptors):
-        """SiftMatch.cpp:110-131: d_descriptors = uint8 cuda tensor [num, 128], normalised to 512.  No copy is made."""
+        """SiftMatch.cpp:110-131: d_descriptors = uint8 cuda tensor [num, 128], normalised to 512.  No copy is made, so the tensor's data must
+        be 16-byte aligned (include/bf_sift.h); a misaligned one makes GetSiftMatch / matchBatch fail with cudaErrorInvalidValue."""
         self._des[index], self._num[index] = d_descriptors, int(num)
 
     def _job(self, des1, n1, des2, n2, ipm: ImagePairMatch, off):

@@ -55,8 +55,25 @@ typedef struct BFSiftMatchJob {
 /* Matches numJobs image pairs (jobs: HOST array) in two launches, asynchronously on the library stream (bfSetStream).
  * Matches are stored in ascending image-2 feature; when a pair has more than 128 the first 128 in that order are kept and the counter holds the
  * total (the reference appends with an atomicAdd: which 128 survive there depends on the scheduling -- this is one of its outcomes, always the same).
- * A job with num1 <= 0 or num2 <= 0 only zeroes its counter (SiftMatch.cpp:162-165).  Returns 0 or a cudaError_t. */
+ * A job with num1 <= 0 or num2 <= 0 only zeroes its counter (SiftMatch.cpp:162-165); its descriptor pointers are not read and may be NULL.
+ * Alignment contract: d_des1 and d_des2 of every other job must be 16-byte aligned (cudaMalloc'd arrays of 128-byte rows are; a uint8 view that
+ * starts at an odd byte is not) -- the reference copies descriptors into its own buffers, this call reads the caller's in 16-byte units.  A batch
+ * that breaks it, or has num1 or num2 >= 2^24, returns cudaErrorInvalidValue before any CUDA call: nothing is enqueued, no counter is touched.
+ * Returns 0 or a cudaError_t. */
 int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distmax, float ratiomax);
+
+/* Sweep of bfSiftMatchBatch, process-wide.  AUTO (the default; BF_SIFT_MATCH=mma in the environment makes MMA the initial setting): the wgmma +
+ * TMA sweep, or the warp-level mma.sync sweep when the driver offers no tensor-map encoder.  WGMMA forces the first: a batch it cannot map
+ * returns cudaErrorNotSupported before anything is enqueued, it never falls back.  MMA forces the second.  Both give the same bytes (counter,
+ * stored indices in storage order, distances); forcing one lets a test compare them.  Returns the previous setting, or cudaErrorInvalidValue
+ * for an unknown one. */
+#define BF_SIFT_SWEEP_AUTO 0
+#define BF_SIFT_SWEEP_WGMMA 1
+#define BF_SIFT_SWEEP_MMA 2
+int bfSiftSetMatchSweep(int sweep);
+/* The last bfSiftMatchBatch that enqueued work, recorded on the host (does not synchronise): out[0] = the sweep that ran (BF_SIFT_SWEEP_WGMMA or
+ * BF_SIFT_SWEEP_MMA; 0 before the first batch), out[1] = its number of jobs. */
+int bfSiftGetMatchInfo(int out[2]);
 
 /* SIFTImageManager::SortKeyPointMatchesCU(curFrame, startFrame, numFrames) (FL/SiftGPU/SIFTImageManager.cu:59-177): sorts the raw matches
  * of every image pair p in [startFrame, numFrames), p != curFrame, by ascending distance, in place.  Arrays are the manager's:

@@ -83,6 +83,21 @@ def test_solver_grid_policy_override_is_checked_on_the_host():
     assert L.bfSolverGetLaunchInfo(C.byref(capi.BFSolverState()), (C.c_int * 4)()) == 1      # no solve on this state
 
 
+def test_sift_match_sweep_switch_is_checked_on_the_host():
+    """bfSiftSetMatchSweep / bfSiftGetMatchInfo are exported; an unknown sweep is refused without a device and leaves the setting as it was"""
+    from bundlefusion_b200 import sift
+    L = capi.lib()
+    assert hasattr(L, "bfSiftSetMatchSweep") and hasattr(L, "bfSiftGetMatchInfo")
+    assert (sift.SIFT_SWEEP_AUTO, sift.SIFT_SWEEP_WGMMA, sift.SIFT_SWEEP_MMA) == (0, 1, 2)
+    prev = L.bfSiftSetMatchSweep(2)
+    assert prev in (0, 2)                                                # auto, or mma when BF_SIFT_MATCH=mma
+    assert L.bfSiftSetMatchSweep(3) == 1 and L.bfSiftSetMatchSweep(-1) == 1      # cudaErrorInvalidValue
+    assert L.bfSiftSetMatchSweep(1) == 2
+    assert L.bfSiftSetMatchSweep(prev) == 1
+    out = (C.c_int * 2)()
+    assert L.bfSiftGetMatchInfo(out) == 0 and out[0] in (0, 1, 2)
+
+
 def test_raycast_pod_layouts():
     assert C.sizeof(capi.BFRayCastParams) == 192 and capi.BFRayCastParams.mx.offset == 128 and capi.BFRayCastParams.m_splatMinimum.offset == 160
     assert capi.BFRayCastParams.m_useGradients.offset == 184 and capi.BFRayCastParams.dummy0.offset == 188       # FL/DepthSensing/CUDARayCastParams.h:8-27
