@@ -24,6 +24,7 @@
 #include "../../include/bf_frameloop.h"
 #include "../../include/bf_host.h"
 #include "../../include/bf_ingest.h"
+#include "../../include/bf_keyframe_search.h"
 #include "../../include/bf_sift.h"
 #include "../../include/bf_solver.h"
 #include "bf_common.cuh"
@@ -1096,6 +1097,19 @@ BF_API int bfFrameLoopGetGlobalProblem(const BFFrameLoop* loop, BFFrameLoopGloba
     out->d_cacheFrames = g.cache.d_frames; out->cacheWidth = g.cache.w; out->cacheHeight = g.cache.h;
     out->intrinsics[0] = g.cache.K[0]; out->intrinsics[1] = g.cache.K[5]; out->intrinsics[2] = g.cache.K[2]; out->intrinsics[3] = g.cache.K[6];
     out->maxNumImages = g.solver.maxImages; out->maxCorrPerImage = g.solver.maxCorrPerImage;
+    return 0;
+}
+
+BF_API int bfFrameLoopGetKeyframes(const BFFrameLoop* loop, BFKeyframeSet* out) {
+    if (!loop || !out) return (int)cudaErrorInvalidValue;
+    const Loop& L = *reinterpret_cast<const Loop*>(loop);
+    const Bundler& g = L.global;
+    memset(out, 0, sizeof(*out));
+    out->numImages = g.sm.numImages; out->maxKeys = g.sm.maxKeys;
+    out->d_keyPoints = g.sm.d_keys; out->d_descriptors = g.sm.d_descs; out->d_numKeys = g.sm.d_numKeys;
+    out->d_cacheFrames = g.cache.d_frames; out->cacheWidth = g.cache.w; out->cacheHeight = g.cache.h;
+    memcpy(out->cacheIntrinsics, g.cache.K, sizeof(out->cacheIntrinsics));
+    memcpy(out->siftIntrinsicsInv, L.siftKinv, sizeof(out->siftIntrinsicsInv));
     return 0;
 }
 

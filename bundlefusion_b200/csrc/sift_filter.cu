@@ -8,6 +8,7 @@
 #include "../../include/bf_sift.h"
 #include "bf_common.cuh"
 #include "mat4.cuh"
+#include "sift_pairs.cuh"
 
 namespace bf {
 
@@ -332,7 +333,7 @@ __device__ unsigned filter_pair(const KeyPoint* kp, uint32_t* idx, float* dist, 
 
 
 struct FilterArgs {
-    unsigned curFrame, startFrame;
+    PairList pl;
     const KeyPoint* kp; const int* numMatches; const float* dists; const uint2* idxs;
     int* numFiltered; float* fDists; uint2* fIdxs; float* fT; float* fTinv;
     float Ki[16]; unsigned minNum; float maxRes2;
@@ -340,8 +341,9 @@ struct FilterArgs {
 
 __global__ void __launch_bounds__(32)
 sift_filter_kernel(const __grid_constant__ FilterArgs a) {
-    const unsigned p = blockIdx.x + a.startFrame, t = threadIdx.x;
-    if (p == a.curFrame) return;
+    const PairRef pr = pair_of(a.pl, blockIdx.x);
+    const unsigned p = pr.slot, t = threadIdx.x;
+    if (pr.skip) return;
     const int raw = a.numMatches[p];
     if (raw <= 0) { if (t == 0) a.numFiltered[p] = 0; return; }                    // SIFTImageManager.cu:211-216
     const unsigned n = (unsigned)min(MAX_RAW, raw);
@@ -372,7 +374,7 @@ sift_filter_kernel(const __grid_constant__ FilterArgs a) {
 }
 
 struct AddArgs {
-    unsigned curFrame, startFrame, numFrames;
+    PairList pl; unsigned numPairs, cap;        // entries at or past cap are counted, not written
     BFEntryJ* glob; uint2* globIdx; int* globNum; const int* numFiltered; const uint2* fIdxs; const KeyPoint* kp;
     const int* lastMatched;           // optional device predicate (bfSiftFilterFrames): nothing is appended when *lastMatched < 0
     float Ki[16];
@@ -403,10 +405,12 @@ sift_add_residuals_kernel(const __grid_constant__ AddArgs a) {
     if (a.lastMatched && *a.lastMatched < 0) return;            // Bundler::matchAndFilter: `if (lastMatchedFrame != -1) AddCurrToResidualsCU(...)`
     if (t == 0) sBase = *a.globNum;
     __syncthreads();
-    for (unsigned p0 = a.startFrame; p0 < a.numFrames; p0 += blockDim.x) {
-        const unsigned p = p0 + t;
+    for (unsigned b0 = 0; b0 < a.numPairs; b0 += blockDim.x) {
+        const unsigned b = b0 + t;
+        const PairRef pr = pair_of(a.pl, b);
+        const unsigned p = pr.slot;
         int cnt = 0;
-        if (p < a.numFrames && p != a.curFrame) cnt = a.numFiltered[p];
+        if (b < a.numPairs && !pr.skip) cnt = a.numFiltered[p];
         sScan[t] = cnt;
         __syncthreads();
         for (unsigned o = 1; o < blockDim.x; o <<= 1) {                 // inclusive Hillis-Steele scan
@@ -419,7 +423,7 @@ sift_add_residuals_kernel(const __grid_constant__ AddArgs a) {
         for (int k = 0; k < cnt; ++k) {
             const uint2 ij = a.fIdxs[(size_t)p * MAX_FILTERED + k];
             BFEntryJ e;
-            e.imgIdx_i = p; e.imgIdx_j = a.curFrame;
+            e.imgIdx_i = pr.i; e.imgIdx_j = pr.j;
             for (int s2 = 0; s2 < 2; ++s2) {
                 const KeyPoint kq = a.kp[s2 == 0 ? ij.x : ij.y];
                 const float v0 = kq.depth * kq.px, v1 = kq.depth * kq.py, v2 = kq.depth * 1.0f;
@@ -428,6 +432,7 @@ sift_add_residuals_kernel(const __grid_constant__ AddArgs a) {
                 o[1] = a.Ki[4] * v0 + a.Ki[5] * v1 + a.Ki[6] * v2 + a.Ki[7];
                 o[2] = a.Ki[8] * v0 + a.Ki[9] * v1 + a.Ki[10] * v2 + a.Ki[11];
             }
+            if ((unsigned)(base + k) >= a.cap) break;
             a.glob[base + k] = e;
             a.globIdx[base + k] = ij;
         }
@@ -451,14 +456,13 @@ BF_API int bfSiftFilterFrames(unsigned int curFrame, unsigned int startFrame, un
     return 0;
 }
 
-static int add_curr_to_residuals(unsigned int curFrame, unsigned int startFrame, unsigned int numFrames, BFEntryJ* d_globMatches,
-                                 uint32_t* d_globMatchesKeyPointIndices, int32_t* d_globNumResiduals, const int32_t* d_currNumFilteredMatchesPerImagePair,
-                                 const uint32_t* d_currFilteredMatchKeyPointIndices, const BFSIFTKeyPoint* d_keyPoints, const float* colorIntrinsicsInv,
-                                 const int32_t* d_lastMatchedFrame) {
-    if (numFrames <= startFrame) return 0;
+int bf::sift_add_pairs(const PairList& L, unsigned nBlocks, BFEntryJ* d_globMatches, uint32_t* d_globMatchesKeyPointIndices, int32_t* d_globNumResiduals,
+                       unsigned cap, const int32_t* d_currNumFilteredMatchesPerImagePair, const uint32_t* d_currFilteredMatchKeyPointIndices,
+                       const BFSIFTKeyPoint* d_keyPoints, const float* colorIntrinsicsInv, const int32_t* d_lastMatchedFrame) {
+    if (!nBlocks) return 0;
     AddArgs a;
     a.lastMatched = d_lastMatchedFrame;
-    a.curFrame = curFrame; a.startFrame = startFrame; a.numFrames = numFrames;
+    a.pl = L; a.numPairs = nBlocks; a.cap = cap;
     a.glob = d_globMatches; a.globIdx = reinterpret_cast<uint2*>(d_globMatchesKeyPointIndices); a.globNum = d_globNumResiduals;
     a.numFiltered = d_currNumFilteredMatchesPerImagePair; a.fIdxs = reinterpret_cast<const uint2*>(d_currFilteredMatchKeyPointIndices);
     a.kp = reinterpret_cast<const KeyPoint*>(d_keyPoints);
@@ -472,8 +476,9 @@ static int add_curr_to_residuals(unsigned int curFrame, unsigned int startFrame,
 BF_API int bfSiftAddCurrToResiduals(unsigned int curFrame, unsigned int startFrame, unsigned int numFrames, BFEntryJ* d_globMatches,
                                     uint32_t* d_globMatchesKeyPointIndices, int32_t* d_globNumResiduals, const int32_t* d_currNumFilteredMatchesPerImagePair,
                                     const uint32_t* d_currFilteredMatchKeyPointIndices, const BFSIFTKeyPoint* d_keyPoints, const float* colorIntrinsicsInv) {
-    return add_curr_to_residuals(curFrame, startFrame, numFrames, d_globMatches, d_globMatchesKeyPointIndices, d_globNumResiduals, d_currNumFilteredMatchesPerImagePair,
-                                 d_currFilteredMatchKeyPointIndices, d_keyPoints, colorIntrinsicsInv, nullptr);
+    if (numFrames <= startFrame) return 0;
+    return sift_add_pairs(frame_pairs(curFrame, startFrame), numFrames - startFrame, d_globMatches, d_globMatchesKeyPointIndices, d_globNumResiduals, 0xFFFFFFFFu,
+                          d_currNumFilteredMatchesPerImagePair, d_currFilteredMatchKeyPointIndices, d_keyPoints, colorIntrinsicsInv, nullptr);
 }
 
 BF_API int bfSiftAddCurrToResidualsIfMatched(unsigned int curFrame, unsigned int startFrame, unsigned int numFrames, BFEntryJ* d_globMatches,
@@ -481,8 +486,9 @@ BF_API int bfSiftAddCurrToResidualsIfMatched(unsigned int curFrame, unsigned int
                                              const uint32_t* d_currFilteredMatchKeyPointIndices, const BFSIFTKeyPoint* d_keyPoints, const float* colorIntrinsicsInv,
                                              const int32_t* d_lastMatchedFrame) {
     if (!d_lastMatchedFrame) return (int)cudaErrorInvalidValue;
-    return add_curr_to_residuals(curFrame, startFrame, numFrames, d_globMatches, d_globMatchesKeyPointIndices, d_globNumResiduals, d_currNumFilteredMatchesPerImagePair,
-                                 d_currFilteredMatchKeyPointIndices, d_keyPoints, colorIntrinsicsInv, d_lastMatchedFrame);
+    if (numFrames <= startFrame) return 0;
+    return sift_add_pairs(frame_pairs(curFrame, startFrame), numFrames - startFrame, d_globMatches, d_globMatchesKeyPointIndices, d_globNumResiduals, 0xFFFFFFFFu,
+                          d_currNumFilteredMatchesPerImagePair, d_currFilteredMatchKeyPointIndices, d_keyPoints, colorIntrinsicsInv, d_lastMatchedFrame);
 }
 
 BF_API int bfSiftFilterKeyPointMatches(unsigned int curFrame, unsigned int startFrame, unsigned int numFrames, const BFSIFTKeyPoint* d_keyPoints,
@@ -491,8 +497,18 @@ BF_API int bfSiftFilterKeyPointMatches(unsigned int curFrame, unsigned int start
                                        float* d_filteredTransforms, float* d_filteredTransformsInv, const float* siftIntrinsicsInv,
                                        unsigned int minNumMatches, float maxKabschRes2) {
     if (numFrames <= startFrame) return 0;                                         // SIFTImageManager.cu:267
+    return sift_filter_pairs(frame_pairs(curFrame, startFrame), numFrames - startFrame, d_keyPoints, d_numMatchesPerImagePair, d_matchDistances, d_matchKeyPointIndices,
+                             d_numFilteredMatchesPerImagePair, d_filteredMatchDistances, d_filteredMatchKeyPointIndices, d_filteredTransforms, d_filteredTransformsInv,
+                             siftIntrinsicsInv, minNumMatches, maxKabschRes2);
+}
+
+int bf::sift_filter_pairs(const PairList& L, unsigned nBlocks, const BFSIFTKeyPoint* d_keyPoints, const int32_t* d_numMatchesPerImagePair, const float* d_matchDistances,
+                          const uint32_t* d_matchKeyPointIndices, int32_t* d_numFilteredMatchesPerImagePair, float* d_filteredMatchDistances,
+                          uint32_t* d_filteredMatchKeyPointIndices, float* d_filteredTransforms, float* d_filteredTransformsInv, const float* siftIntrinsicsInv,
+                          unsigned minNumMatches, float maxKabschRes2) {
+    if (!nBlocks) return 0;
     FilterArgs a;
-    a.curFrame = curFrame; a.startFrame = startFrame;
+    a.pl = L;
     a.kp = reinterpret_cast<const KeyPoint*>(d_keyPoints); a.numMatches = d_numMatchesPerImagePair; a.dists = d_matchDistances;
     a.idxs = reinterpret_cast<const uint2*>(d_matchKeyPointIndices);
     a.numFiltered = d_numFilteredMatchesPerImagePair; a.fDists = d_filteredMatchDistances; a.fIdxs = reinterpret_cast<uint2*>(d_filteredMatchKeyPointIndices);
@@ -500,7 +516,7 @@ BF_API int bfSiftFilterKeyPointMatches(unsigned int curFrame, unsigned int start
     for (int k = 0; k < 16; ++k) a.Ki[k] = siftIntrinsicsInv[k];
     a.minNum = minNumMatches; a.maxRes2 = maxKabschRes2;
     ++g_launchCount;
-    sift_filter_kernel<<<numFrames - startFrame, 32, 0, stream()>>>(a);
+    sift_filter_kernel<<<nBlocks, 32, 0, stream()>>>(a);
     BF_CHECK(cudaGetLastError());
     return 0;
 }

@@ -22,20 +22,12 @@
 
 #include "../../include/bf_sift.h"
 #include "bf_common.cuh"
+#include "sift_pairs.cuh"
+#include "sift_sweep.cuh"
 
 namespace bf {
 
 extern unsigned long long g_launchCount;
-
-struct SiftJobDev {
-    const uint8_t* desA; int nA;       // the features this pass owns ("rows" of the pass)
-    const uint8_t* desB; int nB;       // the features they are compared with
-    int* rowResult; float* rowDist;    // row pass: outputs; column pass: inputs (indexed by image-1 feature)
-    int* numMatches; float* outDist; uint2* outIdx;
-    uint2 offset;
-    int* colResult; int* done;         // column pass: match of each image-2 feature (-1 none), CTAs of the job that have finished
-    const CUtensorMap* mapA; const CUtensorMap* mapB;      // TMA sweep: [n][128 B] tensor maps of the two descriptor arrays (box 128 x 128, 128-byte swizzle, zero fill past n)
-};
 
 // Winner among equal maxima, exactly as the reference's 32 strided lanes + fold-upper-half-into-lower tree pick it (see
 // oracle/sift_oracle.c): smallest (bit-reversed lane, position), lane = col % 32 for rows and (row / 4) % 32 for columns.
@@ -413,9 +405,10 @@ sift_best_wgmma_kernel(const SiftJobDev* __restrict__ jobs, float distmax, float
 // SortKeyPointMatchesCU_Kernel (SIFTImageManager.cu:59-145): one CTA per image pair, 128 slots, bitonic network in shared memory on
 // the total order (distance, image-2 feature, image-1 feature); padding sorts last.
 __global__ void __launch_bounds__(BF_MAX_MATCHES_PER_IMAGE_PAIR_RAW)
-sift_sort_kernel(unsigned curFrame, unsigned startFrame, const int* __restrict__ numMatches, float* dists, uint2* idxs) {
-    const unsigned pair = blockIdx.x + startFrame;
-    if (pair == curFrame) return;
+sift_sort_kernel(const PairList pl, const int* __restrict__ numMatches, float* dists, uint2* idxs) {
+    const PairRef pr = pair_of(pl, blockIdx.x);
+    if (pr.skip) return;
+    const unsigned pair = pr.slot;
     const int n = min(BF_MAX_MATCHES_PER_IMAGE_PAIR_RAW, numMatches[pair]);
     if (n <= 0) return;
     __shared__ float sD[BF_MAX_MATCHES_PER_IMAGE_PAIR_RAW];
@@ -477,21 +470,45 @@ static EncodeTiledFn encode_tiled_fn() {
     return fn;
 }
 // [rows][128] bytes, box 128 bytes x 128 rows, 128-byte swizzle, rows past the end read as zeros
-static bool descriptor_map(const uint8_t* base, int rows, CUtensorMap* out) {
-    auto key = std::make_pair((const void*)base, rows);
-    auto it = g_sift.mapCache.find(key);
-    if (it != g_sift.mapCache.end()) { *out = it->second; return true; }
+bool sift_encode_descriptor_map(const uint8_t* base, int rows, CUtensorMap* out) {
     EncodeTiledFn fn = encode_tiled_fn();
     if (!fn || (reinterpret_cast<uintptr_t>(base) & 15u) || rows <= 0) return false;
     const cuuint64_t dims[2] = { 128, (cuuint64_t)rows }, strides[1] = { 128 };
     const cuuint32_t box[2] = { 128, 128 }, estr[2] = { 1, 1 };
-    if (fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) return false;
+    return fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+static bool descriptor_map(const uint8_t* base, int rows, CUtensorMap* out) {
+    auto key = std::make_pair((const void*)base, rows);
+    auto it = g_sift.mapCache.find(key);
+    if (it != g_sift.mapCache.end()) { *out = it->second; return true; }
+    if (!sift_encode_descriptor_map(base, rows, out)) return false;
     if (g_sift.mapCache.size() > 65536) g_sift.mapCache.clear();
     g_sift.mapCache.emplace(key, *out);
     return true;
 }
 static std::mutex g_siftMutex;
+
+int sift_wgmma_sweep(const SiftJobDev* dJobs, int numJobs, int gx1, int gx2, float distmax, float ratiomax, cudaStream_t s) {
+    if (!g_wgmmaAttrSet) {
+        BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
+        BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
+        g_wgmmaAttrSet = true;
+    }
+    g_launchCount += 2;
+    sift_best_wgmma_kernel<false><<<dim3(gx1, numJobs), 288, TMA_SMEM_BYTES, s>>>(dJobs, distmax, ratiomax);
+    BF_CHECK(cudaGetLastError());
+    sift_best_wgmma_kernel<true><<<dim3(gx2, numJobs), 288, TMA_SMEM_BYTES, s>>>(dJobs + numJobs, distmax, ratiomax);
+    BF_CHECK(cudaGetLastError());
+    return 0;
+}
+int sift_sort_pairs(const PairList& L, unsigned nBlocks, const int32_t* numMatches, float* dists, uint32_t* idxs) {
+    if (!nBlocks) return 0;
+    ++g_launchCount;
+    sift_sort_kernel<<<nBlocks, BF_MAX_MATCHES_PER_IMAGE_PAIR_RAW, 0, stream()>>>(L, numMatches, dists, reinterpret_cast<uint2*>(idxs));
+    BF_CHECK(cudaGetLastError());
+    return 0;
+}
 
 // grows the matcher's scratch to hold `jobs` jobs with `rows` image-1 and `cols` image-2 features in total; `exact`: called with a batch's own numbers
 // (capacities double so that a growing keyframe set rarely reallocates), else a reservation (bfSiftReserveWorkspace: capacities as given)
@@ -565,11 +582,6 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
             return (int)cudaErrorNotSupported;
         }
     }
-    if (useTc && !g_wgmmaAttrSet) {
-        BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
-        BF_CHECK(cudaFuncSetAttribute(sift_best_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_BYTES));
-        g_wgmmaAttrSet = true;
-    }
     cudaStream_t s = stream();
     if (!g_sift.evDone) BF_CHECK(cudaEventCreateWithFlags(&g_sift.evDone, cudaEventDisableTiming));
     BF_CHECK(cudaStreamWaitEvent(s, g_sift.evDone, 0));       // a previous batch (possibly on another stream) still owns rowResult / the job table
@@ -599,15 +611,12 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
     if (useTc) BF_CHECK(cudaMemcpyAsync(g_sift.dMaps, g_sift.hMaps, sizeof(CUtensorMap) * 2 * (size_t)numJobs, cudaMemcpyHostToDevice, s));
     BF_CHECK(cudaMemcpyAsync(g_sift.dJobs, h, sizeof(SiftJobDev) * 2 * (size_t)numJobs, cudaMemcpyHostToDevice, s));
     BF_CHECK(cudaEventRecord(g_sift.evCopied, s));
-    g_launchCount += 2;
     g_matchInfo[0] = useTc ? BF_SIFT_SWEEP_WGMMA : BF_SIFT_SWEEP_MMA; g_matchInfo[1] = numJobs;
     if (useTc) {
         const int gx1 = maxN1 > 0 ? (maxN1 + TC_BM - 1) / TC_BM : 1, gx2 = maxN2 > 0 ? (maxN2 + TC_BM - 1) / TC_BM : 1;
-        sift_best_wgmma_kernel<false><<<dim3(gx1, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs, distmax, ratiomax);
-        BF_CHECK(cudaGetLastError());
-        sift_best_wgmma_kernel<true><<<dim3(gx2, numJobs), 288, TMA_SMEM_BYTES, s>>>(g_sift.dJobs + numJobs, distmax, ratiomax);
-        BF_CHECK(cudaGetLastError());
+        const int rcS = sift_wgmma_sweep(g_sift.dJobs, numJobs, gx1, gx2, distmax, ratiomax, s); if (rcS) return rcS;
     } else {
+        g_launchCount += 2;
         const int gx1 = maxN1 > 0 ? (maxN1 + SM_BM - 1) / SM_BM : 1, gx2 = maxN2 > 0 ? (maxN2 + SM_BM - 1) / SM_BM : 1;
         sift_best_kernel<false><<<dim3(gx1, numJobs), 128, 0, s>>>(g_sift.dJobs, distmax, ratiomax);
         BF_CHECK(cudaGetLastError());
@@ -621,11 +630,7 @@ BF_API int bfSiftMatchBatch(const BFSiftMatchJob* jobs, int numJobs, float distm
 BF_API int bfSiftSortKeyPointMatches(unsigned int curFrame, unsigned int startFrame, unsigned int numFrames, const int32_t* d_numMatchesPerImagePair,
                                      float* d_matchDistances, uint32_t* d_matchKeyPointIndices) {
     if (numFrames <= startFrame) return 0;                                  // SIFTImageManager.cu:148
-    ++g_launchCount;
-    sift_sort_kernel<<<numFrames - startFrame, BF_MAX_MATCHES_PER_IMAGE_PAIR_RAW, 0, stream()>>>(curFrame, startFrame, d_numMatchesPerImagePair, d_matchDistances,
-                                                                                                 reinterpret_cast<uint2*>(d_matchKeyPointIndices));
-    BF_CHECK(cudaGetLastError());
-    return 0;
+    return sift_sort_pairs(frame_pairs(curFrame, startFrame), numFrames - startFrame, d_numMatchesPerImagePair, d_matchDistances, d_matchKeyPointIndices);
 }
 
 BF_API size_t bfSiftWorkspaceBytes(void) {

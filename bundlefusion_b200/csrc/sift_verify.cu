@@ -16,6 +16,7 @@
 #include "../../include/bf_sift.h"
 #include "bf_common.cuh"
 #include "mat4.cuh"
+#include "sift_pairs.cuh"
 
 namespace bf {
 
@@ -89,7 +90,7 @@ __device__ bool eigen_system3(const float m[9], v3 ev[3]) {
 __device__ __forceinline__ float dot3(v3 a, v3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 
 struct AreaArgs {
-    unsigned curFrame, startFrame;
+    PairList pl;
     const KeyPointV* kp; int* numFiltered; const uint2* fIdxs; float* areas;
     float Ki[16]; float areaThresh;
 };
@@ -152,8 +153,9 @@ __device__ float surface_area_one(const AreaArgs& a, const uint2* idx, unsigned 
 
 __global__ void __launch_bounds__(32)
 sift_surface_area_kernel(const __grid_constant__ AreaArgs a) {
-    const unsigned p = blockIdx.x + a.startFrame, lane = threadIdx.x;
-    if (p == a.curFrame) return;
+    const PairRef pr = pair_of(a.pl, blockIdx.x);
+    const unsigned p = pr.slot, lane = threadIdx.x;
+    if (pr.skip) return;
     const int c = a.numFiltered[p];
     if (c <= 0) return;
     const unsigned n = (unsigned)(c < MAX_FILTERED ? c : MAX_FILTERED);
@@ -175,7 +177,7 @@ __device__ __forceinline__ int f2i_gpu(float x) {              // spelled out so
 }
 
 struct VerifyArgs {
-    unsigned curFrame, startFrame, W, H;
+    PairList pl; unsigned W, H;
     int* numFiltered; const float* fT; const BFCUDACachedFrame* frames; float* stats;
     float K[16];
     float distThresh, normalThresh, errThresh, corrThresh, dMin, dMax;
@@ -249,8 +251,9 @@ __device__ __forceinline__ void dense_pair_total(const VerifyArgs& a, const floa
 
 __global__ void __launch_bounds__(1024)
 sift_dense_verify_kernel(const __grid_constant__ VerifyArgs a) {
-    const unsigned p = blockIdx.x + a.startFrame;
-    if (p == a.curFrame) return;
+    const PairRef pr = pair_of(a.pl, blockIdx.x);
+    const unsigned p = pr.slot;
+    if (pr.skip) return;
     if (a.numFiltered[p] == 0) return;
     __shared__ float sT[16], sTinv[16];
     __shared__ float sAdd[64][3];
@@ -260,7 +263,7 @@ sift_dense_verify_kernel(const __grid_constant__ VerifyArgs a) {
     if (t == 0) mat4_inverse_hd(sT, sTinv);
     __syncthreads();
     float err, corr;
-    dense_pair_total(a, sT, sTinv, a.frames[p], a.frames[a.curFrame], sAdd, err, corr);
+    dense_pair_total(a, sT, sTinv, a.frames[pr.i], a.frames[pr.j], sAdd, err, corr);
     if (t == 0) {
         if (a.stats) { a.stats[2 * p] = err; a.stats[2 * p + 1] = corr; }
         if (corr < a.corrThresh || err > a.errThresh || err != err) a.numFiltered[p] = 0;
@@ -304,14 +307,21 @@ BF_API int bfSiftFilterMatchesBySurfaceArea(unsigned int curFrame, unsigned int 
                                             const float* colorIntrinsicsInv, float areaThresh, float* d_areasOut) {
     if (numFrames == 0 || numFrames <= startFrame) return 0;                        // SIFTImageManager.cu:392
     if (!d_keyPoints || !d_currNumFilteredMatchesPerImagePair || !d_currFilteredMatchKeyPointIndices || !colorIntrinsicsInv) return (int)cudaErrorInvalidValue;
+    return sift_surface_area_pairs(frame_pairs(curFrame, startFrame), numFrames - startFrame, d_keyPoints, d_currNumFilteredMatchesPerImagePair,
+                                   d_currFilteredMatchKeyPointIndices, colorIntrinsicsInv, areaThresh, d_areasOut);
+}
+
+int bf::sift_surface_area_pairs(const PairList& L, unsigned nBlocks, const BFSIFTKeyPoint* d_keyPoints, int32_t* d_currNumFilteredMatchesPerImagePair,
+                                const uint32_t* d_currFilteredMatchKeyPointIndices, const float* colorIntrinsicsInv, float areaThresh, float* d_areasOut) {
+    if (!nBlocks) return 0;
     AreaArgs a;
-    a.curFrame = curFrame; a.startFrame = startFrame;
+    a.pl = L;
     a.kp = reinterpret_cast<const KeyPointV*>(d_keyPoints); a.numFiltered = d_currNumFilteredMatchesPerImagePair;
     a.fIdxs = reinterpret_cast<const uint2*>(d_currFilteredMatchKeyPointIndices); a.areas = d_areasOut;
     for (int k = 0; k < 16; ++k) a.Ki[k] = colorIntrinsicsInv[k];
     a.areaThresh = areaThresh;
     ++g_launchCount;
-    sift_surface_area_kernel<<<numFrames - startFrame, 32, 0, stream()>>>(a);
+    sift_surface_area_kernel<<<nBlocks, 32, 0, stream()>>>(a);
     BF_CHECK(cudaGetLastError());
     return 0;
 }
@@ -324,17 +334,26 @@ BF_API int bfSiftFilterMatchesByDenseVerify(unsigned int curFrame, unsigned int 
     if (numFrames == 0 || numFrames <= startFrame) return 0;                        // SIFTImageManager.cu:591
     if (!intrinsics || !d_currNumFilteredMatchesPerImagePair || !d_currFilteredTransforms || !d_cachedFrames || imageWidth == 0 || imageHeight == 0)
         return (int)cudaErrorInvalidValue;
+    const unsigned by = (imageHeight + 31) / 32, nt = imageWidth * by;
+    if (nt % 32 != 0 || nt > 1024) return (int)cudaErrorInvalidValue;             // the reference's block shape; a partial warp in its shuffles is undefined
+    return sift_dense_verify_pairs(frame_pairs(curFrame, startFrame), numFrames - startFrame, imageWidth, imageHeight, intrinsics, d_currNumFilteredMatchesPerImagePair,
+                                   d_currFilteredTransforms, d_cachedFrames, distThresh, normalThresh, errThresh, corrThresh, sensorDepthMin, sensorDepthMax, d_statsOut);
+}
+
+// block shape checked by the caller
+int bf::sift_dense_verify_pairs(const PairList& L, unsigned nBlocks, unsigned imageWidth, unsigned imageHeight, const float* intrinsics,
+                                int32_t* d_currNumFilteredMatchesPerImagePair, const float* d_currFilteredTransforms, const BFCUDACachedFrame* d_cachedFrames,
+                                float distThresh, float normalThresh, float errThresh, float corrThresh, float sensorDepthMin, float sensorDepthMax, float* d_statsOut) {
+    if (!nBlocks) return 0;
     VerifyArgs a;
-    a.curFrame = curFrame; a.startFrame = startFrame; a.W = imageWidth; a.H = imageHeight;
+    a.pl = L; a.W = imageWidth; a.H = imageHeight;
     a.numFiltered = d_currNumFilteredMatchesPerImagePair; a.fT = d_currFilteredTransforms; a.frames = d_cachedFrames; a.stats = d_statsOut;
     for (int k = 0; k < 16; ++k) a.K[k] = intrinsics[k];
     a.distThresh = distThresh; a.normalThresh = normalThresh; a.errThresh = errThresh; a.corrThresh = corrThresh;
     a.dMin = sensorDepthMin; a.dMax = sensorDepthMax;
-    const unsigned by = (imageHeight + 31) / 32, nt = imageWidth * by;
-    if (nt % 32 != 0 || nt > 1024) return (int)cudaErrorInvalidValue;             // the reference's block shape; a partial warp in its shuffles is undefined
     ++g_launchCount;
-    const dim3 block(imageWidth, by);
-    sift_dense_verify_kernel<<<numFrames - startFrame, block, 0, stream()>>>(a);
+    const dim3 block(imageWidth, (imageHeight + 31) / 32);
+    sift_dense_verify_kernel<<<nBlocks, block, 0, stream()>>>(a);
     BF_CHECK(cudaGetLastError());
     return 0;
 }
@@ -347,7 +366,7 @@ BF_API int bfSiftVerifyTrajectory(unsigned int numImages, const int32_t* d_valid
     if (numImages < 2) { set_int_kernel<<<1, 1, 0, stream()>>>(d_validOpt, 0); BF_CHECK(cudaGetLastError()); return 0; }      // SIFTImageManager.cu:1138: returns 0
     if (!d_validImages || !d_trajectory || !intrinsics || !d_cachedFrames || imageWidth == 0 || imageHeight == 0) return (int)cudaErrorInvalidValue;
     TrajVerifyArgs a;
-    a.v.curFrame = 0; a.v.startFrame = 0; a.v.W = imageWidth; a.v.H = imageHeight;
+    a.v.pl = frame_pairs(0, 0); a.v.W = imageWidth; a.v.H = imageHeight;
     a.v.numFiltered = nullptr; a.v.fT = nullptr; a.v.frames = d_cachedFrames; a.v.stats = d_statsOut;
     for (int k = 0; k < 16; ++k) a.v.K[k] = intrinsics[k];
     a.v.distThresh = distThresh; a.v.normalThresh = normalThresh; a.v.errThresh = errThresh; a.v.corrThresh = corrThresh;

@@ -88,6 +88,7 @@ def _bind(L):
     L.bfFrameLoopStepPastEnd.argtypes = [vp, C.POINTER(BFFrameLoopStatus)]
     L.bfFrameLoopFinish.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(BFFrameLoopFinishInfo)]
     L.bfFrameLoopGetGlobalProblem.argtypes = [vp, C.POINTER(BFFrameLoopGlobalProblem)]
+    L.bfFrameLoopGetKeyframes.argtypes = [vp, vp]
     L.bfFrameLoopGetTrajectory.argtypes = [vp, vp, C.c_uint]
     L.bfFrameLoopGetTrajectory.restype = C.c_uint
     L.bfFrameLoopGetHashData.argtypes = [vp]
@@ -172,6 +173,13 @@ class FrameLoop:
         out = BFFrameLoopGlobalProblem()
         capi.check(self.lib.bfFrameLoopGetGlobalProblem(self._h, C.byref(out)), "bfFrameLoopGetGlobalProblem")
         return out
+
+    def keyframes(self):
+        """the global SIFT manager's keyframe set as keyframe_search.KeyframeSet (views of the loop's device memory, valid until the next loop call)"""
+        from .keyframe_search import BFKeyframeSet, KeyframeSet
+        out = BFKeyframeSet()
+        capi.check(self.lib.bfFrameLoopGetKeyframes(self._h, C.byref(out)), "bfFrameLoopGetKeyframes")
+        return KeyframeSet.from_struct(out, self.device, owner=self)
 
     def trajectory(self, n: int) -> np.ndarray:
         out = np.zeros((n, 4, 4), np.float32)

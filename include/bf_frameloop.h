@@ -33,6 +33,7 @@
 #include <stdint.h>
 
 #include "bf_host.h"
+#include "bf_keyframe_search.h"
 #include "bf_solver.h"
 #include "bf_tsdf.h"
 
@@ -165,6 +166,9 @@ typedef struct BFFrameLoopGlobalProblem {
     uint32_t maxCorrPerImage;
 } BFFrameLoopGlobalProblem;
 int bfFrameLoopGetGlobalProblem(const BFFrameLoop* loop, BFFrameLoopGlobalProblem* out);
+/* The global (keyframe) SIFT manager's keyframe set -- keys, descriptors, key counts, cache frames, cache size and intrinsics, the inverse SIFT
+ * intrinsics -- as bfKeyframeSearch reads it: the loop's own device pointers, valid until the next loop call.  Nothing in the loop changes. */
+int bfFrameLoopGetKeyframes(const BFFrameLoop* loop, BFKeyframeSet* out);
 
 /* optimised camera-to-world poses of the first n frames (host, [n][16]; invalid frames all -inf); returns the number written */
 unsigned int bfFrameLoopGetTrajectory(BFFrameLoop* loop, float* h_out, unsigned int maxFrames);
