@@ -104,6 +104,7 @@ TSDF_SYMBOLS = [
     "bfSetStream", "bfGetStream", "bfGetLastErrorString", "bfTsdfAuxBytes", "bfTsdfReset", "bfTsdfIntegrateFrame",
     "bfTsdfGarbageCollect", "bfTsdfGetHeapFreeCount", "bfTsdfGetNumOccupiedBlocks", "bfTsdfGetLastFrameStats",
     "bfTsdfReleaseAux", "bfTsdfReintegrateFrame", "bfGetLaunchCount", "bfTsdfSetProfiling", "bfTsdfGetProfile", "bfTsdfGetProfileEx", "bfTsdfSetLanes", "bfTsdfSetArithmetic", "bfTsdfReintegrateBatch", "bfTsdfSetBatching",
+    "bfTsdfIntegrateBatch",
 ]
 
 HOST_SYMBOLS = ["bfMat4Inverse", "bfTsdfRunOps"]
@@ -314,6 +315,7 @@ def lib() -> C.CDLL:
     L.bfMat4Inverse.argtypes = [P(C.c_float), P(C.c_float)]
     L.bfMat4Inverse.restype = None
     L.bfTsdfRunOps.argtypes = [P(BFHashDataStruct), P(BFHashParams), P(BFDepthCameraParams), P(BFTsdfOp), C.c_int, P(vp), P(vp)]
+    L.bfTsdfIntegrateBatch.argtypes = [P(BFHashDataStruct), P(BFHashParams), P(BFDepthCameraParams), vp, vp, C.c_int, vp, vp]
     # solver
     L.solveBundlingStub.argtypes = [P(BFSolverInput), P(BFSolverState), P(BFSolverParameters), P(BFSolverStateAnalysis), P(C.c_float), vp]
     L.solveBundlingStub.restype = None

@@ -31,6 +31,7 @@
 #include "mat4.cuh"
 
 namespace bf {
+int tsdf_batching_usable();          // tsdf.cu: batching on and fast arithmetic selected (bfTsdfRunOps' rule)
 
 extern unsigned long long g_launchCount;
 
@@ -1085,6 +1086,53 @@ BF_API int bfFrameLoopFinish(BFFrameLoop* loop, uint32_t numSolveFramesBeforeExi
         info->done = L.finished ? 1 : 0;
     }
     return L.finished ? 0 : (int)cudaErrorNotReady;
+}
+
+BF_API int bfFrameLoopFuse(BFFrameLoop* loop, BFHashDataStruct* hd, BFHashParams* hp, const float* h_poses, uint32_t numFrames, BFFrameLoopFuseInfo* info) {
+    if (!loop || !hd || !hp) return (int)cudaErrorInvalidValue;
+    Loop& L = *reinterpret_cast<Loop*>(loop);
+    if (L.ahead.valid) { set_last_error("bfFrameLoopFuse: a frame announced by bfFrameLoopStepAhead is still pending", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    if (numFrames > L.numFrames) { set_last_error("bfFrameLoopFuse: numFrames exceeds the frames stepped", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    if (hd->d_hash == L.hd.d_hash) { set_last_error("bfFrameLoopFuse: the target is the loop's own voxel hash", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    std::vector<float> traj;
+    if (!h_poses) {
+        traj.assign((size_t)std::max(L.P.maxNumFrames, numFrames) * 16, kNegInf);
+        bfTrajectoryGetOptimizedTransforms(L.tm, traj.data());          // frames it has no pose for stay -inf: skipped
+        h_poses = traj.data();
+    }
+    FL_OK(join_tsdf(L));
+    const bool batch = tsdf_batching_usable() != 0;
+    BFFrameLoopFuseInfo fi; memset(&fi, 0, sizeof(fi));
+    int32_t frames[16]; float poses[16 * 16];
+    std::vector<BFTsdfOp> ops;
+    unsigned n = 0;
+    for (uint32_t f = 0; f <= numFrames; ++f) {
+        if (f < numFrames) {
+            const float* T = h_poses + 16 * (size_t)f;
+            bool finite = true;
+            for (int e = 0; e < 16; ++e) finite = finite && std::isfinite(T[e]);
+            if (!finite) { ++fi.framesSkipped; continue; }
+            frames[n] = (int32_t)f; memcpy(poses + 16 * n, T, 64); ++n;
+            if (n < 16) continue;
+        }
+        if (n == 0) continue;
+        if (batch) {
+            FL_OK(bfTsdfIntegrateBatch(hd, hp, &L.cam, frames, poses, (int)n, L.depthPtrs.data(), L.colorPtrs.data()));
+            FL_OK(bfTsdfGarbageCollect(hd, hp));
+        } else {
+            ops.assign(n + 1, BFTsdfOp{});
+            for (unsigned k = 0; k < n; ++k) { ops[k].kind = BF_TSDF_OP_INTEGRATE; ops[k].frame = frames[k]; memcpy(ops[k].pose, poses + 16 * k, 64); }
+            ops[n].kind = BF_TSDF_OP_GARBAGE_COLLECT;
+            FL_OK(bfTsdfRunOps(hd, hp, &L.cam, ops.data(), (int)ops.size(), L.depthPtrs.data(), L.colorPtrs.data()));
+        }
+        fi.framesFused += n; ++fi.batches; n = 0;
+    }
+    unsigned long long st[4] = { 0, 0, 0, 0 };
+    if (fi.batches) FL_OK(bfTsdfGetLastFrameStats(hd, st));
+    fi.insertsDropped = st[3];
+    FL_OK(bfTsdfGetHeapFreeCount(hd, &fi.heapFreeCount));
+    if (info) *info = fi;
+    return 0;
 }
 
 BF_API int bfFrameLoopGetGlobalProblem(const BFFrameLoop* loop, BFFrameLoopGlobalProblem* out) {

@@ -891,7 +891,9 @@ compactify_dual_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams
 // one union list: per allocated block the 2-bit-per-op mask {in the old pose's frustum, in the new pose's frustum} for the ops that saw
 // the block exist (op index >= the block's tag; a block inserted by op j's alloc does not exist for ops < j in the reference's order),
 // and the multi-op stencil (tsdf_fast.cu) applies the ops to each voxel in order, in registers: one voxel read and write for the batch.
+// kOldPose = false (bfTsdfIntegrateBatch): integrations only -- no op has an old pose, so no old frustum is tested and no bit 0 is set.
 struct MultiFrusta { int nOps; float voxelSize; float truncScale, truncation; int tilesX; unsigned tilesPerOp; BFFloat4x4 inv[2 * BF_MULTI_MAX_OPS]; };     // inv[2k] = old pose of op k (inverse), inv[2k+1] = new
+template <bool kOldPose>
 __global__ void __launch_bounds__(256)
 compactify_multi_kernel(BFHashDataStruct hd, const __grid_constant__ MultiFrusta fr, const __grid_constant__ BFDepthCameraParams cp,
                         const int4* __restrict__ slotInfo, const unsigned* __restrict__ slotEpoch, unsigned batchId, unsigned* ctrs, int set,
@@ -917,7 +919,7 @@ compactify_multi_kernel(BFHashDataStruct hd, const __grid_constant__ MultiFrusta
                 const int first = ((e >> 8) == batchId) ? (int)(e & 0xffu) : 0;
                 for (int k = first; k < fr.nOps; ++k) {
                     const float2* const tk = tiles ? tiles + (size_t)k * fr.tilesPerOp : nullptr;
-                    if (block_in_frustum_m(fr.voxelSize, fr.inv[2 * k], cp, b)) {
+                    if (kOldPose && block_in_frustum_m(fr.voxelSize, fr.inv[2 * k], cp, b)) {
                         mask |= 1u << (2 * k);
                         if (!tk || block_can_pass_m(fr.truncScale, fr.truncation, fr.voxelSize, fr.inv[2 * k], cp, tk, fr.tilesX, b)) wmask |= 1u << (2 * k);
                     }
@@ -937,7 +939,7 @@ compactify_multi_kernel(BFHashDataStruct hd, const __grid_constant__ MultiFrusta
             // Work order: a block's cost grows with the number of (op, pose) probes it takes -- up to 2 nOps of them, ~60 k cycles for a CTA at
             // 20.  Items go to four buckets by cost quartile and the stencil deals the costliest bucket first (longest-processing-time-first), so
             // the kernel ends on cheap blocks and its tail is a quartile-0 block, not a 20-probe one.
-            const unsigned n2 = 2u * (unsigned)fr.nOps;
+            const unsigned n2 = (kOldPose ? 2u : 1u) * (unsigned)fr.nOps;
             const int q = (wmask == 0) ? -1 : (4u * bits > 3u * n2 ? 3 : (2u * bits > n2 ? 2 : (4u * bits > n2 ? 1 : 0)));
             const unsigned b3 = __ballot_sync(0xffffffffu, q == 3), b2 = __ballot_sync(0xffffffffu, q == 2), b1 = __ballot_sync(0xffffffffu, q == 1), b0 = __ballot_sync(0xffffffffu, q == 0);
             unsigned warpBase = 0, base3 = 0, base2 = 0, base1 = 0, base0 = 0;
@@ -1423,11 +1425,11 @@ BF_API int bfTsdfReintegrateFrame(BFHashDataStruct* hd, const BFHashParams* hpOl
 }
 
 // Up to BF_MULTI_MAX_OPS re-integration pairs {deIntegrate(frame f, old pose); integrate(frame f, new pose)} -- the loop body of
-// FL/DepthSensing/DepthSensing.cpp:867-895, replayed as: n alloc launches (op-tagged inserts), ONE union list, ONE stencil pass in which
-// every voxel of the list is read once, taken through the n pairs in order in registers, and written once.  Fast arithmetic only (the
-// bit-exact kernels keep the one-pair-per-pass path); voxels are bit-identical to the one-pair-per-pass fast path (same probe expression,
-// same per-voxel op order, blocks invisible to the ops that precede their insertion).  hp: pose-independent parameters; on return it holds
-// the last new pose, as after the reference's last integrate.
+// FL/DepthSensing/DepthSensing.cpp:867-895 -- or integrations {integrate(frame f, pose)}, replayed as: n alloc launches (op-tagged inserts), ONE
+// union list, ONE stencil pass in which every voxel of the list is read once, taken through the n ops in order in registers, and written once.
+// Fast arithmetic only (the bit-exact kernels keep the one-op-per-pass path); voxels are bit-identical to the one-op-per-pass fast path (same
+// probe expression, same per-voxel update and op order, blocks invisible to the ops that precede their insertion).  hp: pose-independent
+// parameters; on return it holds the last new pose, as after the reference's last integrate.
 static int g_batching = -1;
 static bool batching_on() {
     if (g_batching < 0) { const char* e = getenv("BF_TSDF_BATCH"); g_batching = (e && e[0] == '0') ? 0 : 1; }
@@ -1435,9 +1437,12 @@ static bool batching_on() {
 }
 BF_API int bfTsdfSetBatching(int enable) { const int prev = batching_on() ? 1 : 0; g_batching = enable ? 1 : 0; return prev; }
 
-BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraParams* cp, const BFTsdfReintegration* pairs, int numPairs,
-                                  const float* const* d_depthFrames, const uint8_t* const* d_colorFrames) {
-    if (numPairs < 1 || numPairs > BF_MULTI_MAX_OPS || !d_colorFrames) return (int)cudaErrorInvalidValue;
+// oldPoses[k] NULL for every k: an integration-only batch.  Every argument is checked before anything is enqueued.
+static int run_batch(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraParams* cp, int n, const int32_t* frames, const float* const* oldPoses,
+                     const float* const* newPoses, const float* const* d_depthFrames, const uint8_t* const* d_colorFrames) {
+    if (n < 1 || n > BF_MULTI_MAX_OPS || !d_depthFrames || !d_colorFrames) return (int)cudaErrorInvalidValue;
+    for (int k = 0; k < n; ++k)
+        if (frames[k] < 0 || !d_depthFrames[frames[k]] || !d_colorFrames[frames[k]]) return (int)cudaErrorInvalidValue;
     TsdfAux* aux;
     int rc = get_aux(hd, hp, &aux, true);
     if (rc) return rc;
@@ -1452,10 +1457,11 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
     rc = join_lanes(aux); if (rc) return rc;            // the batch runs on the caller's stream, after every stencil in flight
     aux->batchId = (aux->batchId + 1u) & 0x00FFFFFFu;
     if (aux->batchId == 0) { BF_CHECK(cudaMemsetAsync(aux->slotEpoch, 0, sizeof(unsigned) * (size_t)aux->numSlots, g_stream)); aux->batchId = 1; }
+    const bool oldPose = oldPoses[0] != nullptr;
     static BFHashParams hpOld[BF_MULTI_MAX_OPS], hpNew[BF_MULTI_MAX_OPS];
     static MultiFrusta fr;
     BFMultiOpDesc desc[BF_MULTI_MAX_OPS];
-    fr.nOps = numPairs; fr.voxelSize = hp->m_virtualVoxelSize; fr.truncScale = hp->m_truncScale; fr.truncation = hp->m_truncation;
+    fr.nOps = n; fr.voxelSize = hp->m_virtualVoxelSize; fr.truncScale = hp->m_truncScale; fr.truncation = hp->m_truncation;
     fr.tilesX = tiles_x(cp); fr.tilesPerOp = (unsigned)(tiles_x(cp) * tiles_y(cp));
     if (aux->tilesMultiPer < fr.tilesPerOp) {
         if (aux->tilesMulti) { BF_CHECK(cudaStreamSynchronize(g_stream)); BF_CHECK(cudaFree(aux->tilesMulti)); aux->tilesMulti = nullptr; aux->tilesMultiPer = 0; }
@@ -1463,15 +1469,20 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
         aux->tilesMultiPer = fr.tilesPerOp;
     }
     const unsigned newParity = aux->parity ^ 1u;
-    for (int k = 0; k < numPairs; ++k) {
-        hpOld[k] = *hp; hpNew[k] = *hp;
-        for (int e = 0; e < 16; ++e) { hpOld[k].m_rigidTransform.m[e] = pairs[k].oldPose[e]; hpNew[k].m_rigidTransform.m[e] = pairs[k].newPose[e]; }
-        mat4_inverse_ref(pairs[k].oldPose, hpOld[k].m_rigidTransformInverse.m);          // as setLastRigidTransform forms it on the reference's host
-        mat4_inverse_ref(pairs[k].newPose, hpNew[k].m_rigidTransformInverse.m);
-        fr.inv[2 * k] = hpOld[k].m_rigidTransformInverse; fr.inv[2 * k + 1] = hpNew[k].m_rigidTransformInverse;
-        desc[k].hpOld = &hpOld[k]; desc[k].hpNew = &hpNew[k];
-        desc[k].depth = d_depthFrames[pairs[k].frame]; desc[k].color = d_colorFrames[pairs[k].frame];
-        if (!desc[k].color || !desc[k].depth) return (int)cudaErrorInvalidValue;
+    for (int k = 0; k < n; ++k) {
+        hpNew[k] = *hp;
+        for (int e = 0; e < 16; ++e) hpNew[k].m_rigidTransform.m[e] = newPoses[k][e];
+        mat4_inverse_ref(newPoses[k], hpNew[k].m_rigidTransformInverse.m);          // as setLastRigidTransform forms it on the reference's host
+        fr.inv[2 * k + 1] = hpNew[k].m_rigidTransformInverse;
+        desc[k].hpOld = nullptr; desc[k].hpNew = &hpNew[k];
+        if (oldPose) {
+            hpOld[k] = *hp;
+            for (int e = 0; e < 16; ++e) hpOld[k].m_rigidTransform.m[e] = oldPoses[k][e];
+            mat4_inverse_ref(oldPoses[k], hpOld[k].m_rigidTransformInverse.m);
+            fr.inv[2 * k] = hpOld[k].m_rigidTransformInverse;
+            desc[k].hpOld = &hpOld[k];
+        }
+        desc[k].depth = d_depthFrames[frames[k]]; desc[k].color = d_colorFrames[frames[k]];
         // the first alloc launch also zeroes the counter set the list is about to use
         rc = do_alloc(hd, &hpNew[k], desc[k].depth, cp, aux, k == 0 ? (int)newParity : -1, AllocEpoch{aux->slotEpoch, (aux->batchId << 8) | (unsigned)k},
                       aux->tilesMulti + (size_t)k * fr.tilesPerOp);
@@ -1481,17 +1492,33 @@ BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const 
     aux->lastListDual = true;
     const int set = set_of(aux->parity);
     ++g_launchCount;
-    compactify_multi_kernel<<<grid_for((hp->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(*hd, fr, *cp, aux->slotInfo, aux->slotEpoch, aux->batchId, aux->ctrs, set,
-                                                                                                 aux->listFlags, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots,
-                                                                                                 aux->tilesMulti);
+    (oldPose ? compactify_multi_kernel<true> : compactify_multi_kernel<false>)<<<grid_for((hp->m_numSDFBlocks + 255) / 256, 4), 256, 0, g_stream>>>(
+        *hd, fr, *cp, aux->slotInfo, aux->slotEpoch, aux->batchId, aux->ctrs, set, aux->listFlags, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u],
+        aux->workMask, aux->workMask2, aux->numSlots, aux->tilesMulti);
     BF_CHECK(cudaGetLastError());
-    rc = profiled_launch(g_stream, true, (unsigned)numPairs, [&](unsigned long long* ktime) {
-        return launch_reintegrate_multi_fast(hd, desc, numPairs, cp, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots, set,
-                                             aux->ctrs, aux->live, grid_for(hp->m_numSDFBlocks, fast_stencil_ctas_per_sm(true)), g_stream, ktime);
+    rc = profiled_launch(g_stream, true, (unsigned)n, [&](unsigned long long* ktime) {
+        return launch_reintegrate_multi_fast(hd, desc, n, cp, aux->work2[aux->parity], aux->work2[aux->parity ^ 1u], aux->workMask, aux->workMask2, aux->numSlots, set,
+                                             aux->ctrs, aux->live, grid_for(hp->m_numSDFBlocks, fast_stencil_ctas_per_sm(oldPose)), g_stream, ktime);
     });
     if (rc) return rc;
-    *hp = hpNew[numPairs - 1];
+    *hp = hpNew[n - 1];
     return 0;
+}
+
+BF_API int bfTsdfReintegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraParams* cp, const BFTsdfReintegration* pairs, int numPairs,
+                                  const float* const* d_depthFrames, const uint8_t* const* d_colorFrames) {
+    if (numPairs < 1 || numPairs > BF_MULTI_MAX_OPS || !pairs) return (int)cudaErrorInvalidValue;
+    int32_t frames[BF_MULTI_MAX_OPS]; const float* oldPoses[BF_MULTI_MAX_OPS]; const float* newPoses[BF_MULTI_MAX_OPS];
+    for (int k = 0; k < numPairs; ++k) { frames[k] = pairs[k].frame; oldPoses[k] = pairs[k].oldPose; newPoses[k] = pairs[k].newPose; }
+    return run_batch(hd, hp, cp, numPairs, frames, oldPoses, newPoses, d_depthFrames, d_colorFrames);
+}
+
+BF_API int bfTsdfIntegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const BFDepthCameraParams* cp, const int32_t* frames, const float* poses, int n,
+                                const float* const* d_depthFrames, const uint8_t* const* d_colorFrames) {
+    if (n < 1 || n > BF_MULTI_MAX_OPS || !frames || !poses) return (int)cudaErrorInvalidValue;
+    const float* oldPoses[BF_MULTI_MAX_OPS]; const float* newPoses[BF_MULTI_MAX_OPS];
+    for (int k = 0; k < n; ++k) { oldPoses[k] = nullptr; newPoses[k] = poses + 16 * (size_t)k; }
+    return run_batch(hd, hp, cp, n, frames, oldPoses, newPoses, d_depthFrames, d_colorFrames);
 }
 namespace bf { int tsdf_batching_usable() { return (batching_on() && arith_fast()) ? 1 : 0; } }
 

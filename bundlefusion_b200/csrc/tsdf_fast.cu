@@ -257,7 +257,10 @@ __device__ __forceinline__ void process_block(const FastArgs& a, const ThreadVox
     live_delta_commit(a.live, ptr / BF_SDF_BLOCK_VOXELS, t, liveDelta);
 }
 
-// one SDF block of a batch: the ops whose mask bits are set are applied in order to the voxel quad held in registers
+// one SDF block of a batch: the ops whose mask bits are set are applied in order to the voxel quad held in registers.  kOldPose = false: a batch of
+// integrations only (bfTsdfIntegrateBatch) -- no op has an old pose, its mask bit 0 is never set, and each passing voxel takes integrate_fast, the
+// very update the one-frame stencil (MODE 0) applies, so the batch is bit-identical to the frames integrated one by one
+template <bool kOldPose>
 __device__ __forceinline__ void process_block_multi(const MultiArgs& a, const ThreadVoxel& o, unsigned t, int4 w, unsigned opMask, unsigned& passed) {
     const float vx = (float)(w.x * BF_SDF_BLOCK_SIZE + o.lx), vy = (float)(w.y * BF_SDF_BLOCK_SIZE + o.ly), vz = (float)(w.z * BF_SDF_BLOCK_SIZE + o.lz);
     uint4* const vp = reinterpret_cast<uint4*>(a.blocks + (size_t)(unsigned)w.w * BF_SDF_BLOCK_VOXELS) + 3 * t;
@@ -267,29 +270,36 @@ __device__ __forceinline__ void process_block_multi(const MultiArgs& a, const Th
     int liveDelta = 0;
 #pragma unroll 1
     for (int k = 0; k < a.nOps; ++k) {
-        const unsigned fl = (opMask >> (2 * k)) & 3u;
+        const unsigned fl = (opMask >> (2 * k)) & (kOldPose ? 3u : 2u);
         if (!fl) continue;                                   // uniform for the CTA
         const MultiOp& op = a.ops[k];
         ProbeSet pA, pB;
         float zA[4], zB[4];
         pA.mask = 0; pB.mask = 0;
-        if (fl & 1u) project4(a.cam, op.depth, op.A, vx, vy, vz, pA, zA);
+        if (kOldPose && (fl & 1u)) project4(a.cam, op.depth, op.A, vx, vy, vz, pA, zA);
         if (fl & 2u) project4(a.cam, op.depth, op.B, vx, vy, vz, pB, zB);
-        if (fl & 1u) decide4(op.A, pA, zA);
+        if (kOldPose && (fl & 1u)) decide4(op.A, pA, zA);
         if (fl & 2u) decide4(op.B, pB, zB);
         const unsigned mask = pA.mask | pB.mask;
         if (mask) {
             unsigned cA[4], cB[4];
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                cA[j] = __ldg(&op.color[(pA.mask >> j) & 1u ? pA.idx[j] : 0u]);
+                cA[j] = kOldPose ? __ldg(&op.color[(pA.mask >> j) & 1u ? pA.idx[j] : 0u]) : 0u;
                 cB[j] = __ldg(&op.color[(pB.mask >> j) & 1u ? pB.idx[j] : 0u]);
             }
             if (!loaded) { qa = vp[0]; qb = vp[1]; qc = vp[2]; loaded = true; }
-            if (mask & 1u) update_pair(op.B, pA.mask & 1u, pA.sdf[0], cA[0], pB.mask & 1u, pB.sdf[0], cB[0], qa.x, qa.y, qa.z, liveDelta);
-            if (mask & 2u) update_pair(op.B, pA.mask & 2u, pA.sdf[1], cA[1], pB.mask & 2u, pB.sdf[1], cB[1], qa.w, qb.x, qb.y, liveDelta);
-            if (mask & 4u) update_pair(op.B, pA.mask & 4u, pA.sdf[2], cA[2], pB.mask & 4u, pB.sdf[2], cB[2], qb.z, qb.w, qc.x, liveDelta);
-            if (mask & 8u) update_pair(op.B, pA.mask & 8u, pA.sdf[3], cA[3], pB.mask & 8u, pB.sdf[3], cB[3], qc.y, qc.z, qc.w, liveDelta);
+            if (kOldPose) {
+                if (mask & 1u) update_pair(op.B, pA.mask & 1u, pA.sdf[0], cA[0], pB.mask & 1u, pB.sdf[0], cB[0], qa.x, qa.y, qa.z, liveDelta);
+                if (mask & 2u) update_pair(op.B, pA.mask & 2u, pA.sdf[1], cA[1], pB.mask & 2u, pB.sdf[1], cB[1], qa.w, qb.x, qb.y, liveDelta);
+                if (mask & 4u) update_pair(op.B, pA.mask & 4u, pA.sdf[2], cA[2], pB.mask & 4u, pB.sdf[2], cB[2], qb.z, qb.w, qc.x, liveDelta);
+                if (mask & 8u) update_pair(op.B, pA.mask & 8u, pA.sdf[3], cA[3], pB.mask & 8u, pB.sdf[3], cB[3], qc.y, qc.z, qc.w, liveDelta);
+            } else {
+                if (mask & 1u) update_fast<0>(op.B, op.B, true, pB.sdf[0], cB[0], false, 0.0f, 0u, qa.x, qa.y, qa.z, liveDelta);
+                if (mask & 2u) update_fast<0>(op.B, op.B, true, pB.sdf[1], cB[1], false, 0.0f, 0u, qa.w, qb.x, qb.y, liveDelta);
+                if (mask & 4u) update_fast<0>(op.B, op.B, true, pB.sdf[2], cB[2], false, 0.0f, 0u, qb.z, qb.w, qc.x, liveDelta);
+                if (mask & 8u) update_fast<0>(op.B, op.B, true, pB.sdf[3], cB[3], false, 0.0f, 0u, qc.y, qc.z, qc.w, liveDelta);
+            }
             dirty |= mask;
             passed += __popc(pA.mask) + __popc(pB.mask);
         }
@@ -366,8 +376,10 @@ stencil_fast_kernel(const __grid_constant__ FastArgs a) {
 #endif
 }
 
-// batch re-integration: the same persistent grid and dynamic deal over the union list, every block visited once for up to 16 ops
-__global__ void __launch_bounds__(128, BF_FAST_MINBLOCKS_FUSED)
+// batch re-integration (kOldPose) or batch integration: the same persistent grid and dynamic deal over the union list, every block visited once
+// for up to 16 ops
+template <bool kOldPose>
+__global__ void __launch_bounds__(128, kOldPose ? BF_FAST_MINBLOCKS_FUSED : BF_FAST_MINBLOCKS)
 stencil_multi_kernel(const __grid_constant__ MultiArgs a) {
     // ticket i -> work item: the four cost buckets in order, costliest first (layout: tsdf_shared.cuh)
     const unsigned n3 = a.ctrs[a.set + SET_WORK], n2 = a.ctrs[a.set + SET_Q2], n1 = a.ctrs[a.set + SET_Q1], n0 = a.ctrs[a.set + SET_Q0];
@@ -403,7 +415,7 @@ stencil_multi_kernel(const __grid_constant__ MultiArgs a) {
     }
     unsigned parity = 0;
     while (wCur.w != -1) {
-        process_block_multi(a, o, t, wCur, mCur, passed);
+        process_block_multi<kOldPose>(a, o, t, wCur, mCur, passed);
         if (t == 0) {
             sWork[parity] = wNext; sMask[parity] = mNext;
             wNext = kEnd; mNext = 0;
@@ -422,7 +434,7 @@ stencil_multi_kernel(const __grid_constant__ MultiArgs a) {
     }
     if (a.ktime && t == 0) { unsigned long long g; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g)); atomicMax(&a.ktime[1], g); }
 #else
-    for (unsigned b = blockIdx.x; b < count; b += gridDim.x) { int4 w; unsigned m; BF_MULTI_LOAD(b, w, m); process_block_multi(a, o, t, w, m, passed); }
+    for (unsigned b = blockIdx.x; b < count; b += gridDim.x) { int4 w; unsigned m; BF_MULTI_LOAD(b, w, m); process_block_multi<kOldPose>(a, o, t, w, m, passed); }
     if (passed) { atomicAdd(reinterpret_cast<unsigned long long*>(&a.ctrs[a.set + SET_U_LO]), (unsigned long long)passed); atomicAdd(reinterpret_cast<unsigned long long*>(&a.ctrs[CTR_U_TOT_LO]), (unsigned long long)passed); }
 #endif
 #undef BF_MULTI_LOAD
@@ -480,10 +492,14 @@ int launch_reintegrate_multi_fast(const BFHashDataStruct* hd, const BFMultiOpDes
     a.blocks = hd->d_SDFBlocks; a.workA = workA; a.workB = workB; a.maskA = maskA; a.maskB = maskB; a.ctrs = ctrs; a.live = live; a.listCounterOut = hd->d_hashCompactifiedCounter;
     a.set = set; a.nOps = nOps; a.workCap = workCap; a.ktime = ktime;
     a.cam.W = cp->m_imageWidth; a.cam.H = cp->m_imageHeight; a.cam.fx = cp->fx; a.cam.fy = cp->fy; a.cam.mx5 = cp->mx + 0.5f; a.cam.my5 = cp->my + 0.5f;
+    const bool oldPose = ops[0].hpOld != nullptr;     // all ops of a batch alike: re-integration pairs, or integrations (hpOld NULL)
     for (int k = 0; k < nOps; ++k) {
-        make_pose(ops[k].hpOld, cp, &a.ops[k].A); make_pose(ops[k].hpNew, cp, &a.ops[k].B);
+        make_pose(ops[k].hpNew, cp, &a.ops[k].B);
+        if (oldPose) make_pose(ops[k].hpOld, cp, &a.ops[k].A); else a.ops[k].A = a.ops[k].B;
         a.ops[k].depth = ops[k].depth; a.ops[k].color = reinterpret_cast<const unsigned*>(ops[k].color);
     }
+    // one launch site for both instantiations, under the kernel's name: tests/test_tsdf_fast_emulated.py rewrites this launch to run the kernel on the CPU
+    void (*const stencil_multi_kernel)(MultiArgs) = oldPose ? bf::stencil_multi_kernel<true> : bf::stencil_multi_kernel<false>;
     stencil_multi_kernel<<<grid, 128, 0, s>>>(a);
     BF_CHECK(cudaGetLastError());
     return 0;

@@ -23,7 +23,8 @@ int launch_reintegrate_fast(const BFHashDataStruct* hd, const BFHashParams* hpOl
                             const float* depth, const void* color, const int4* work, int set, unsigned* ctrs, int* live, int grid, cudaStream_t s);
 int fast_stencil_ctas_per_sm(bool fused);
 
-// batch re-integration: up to BF_MULTI_MAX_OPS (old pose, new pose, frame) triples applied to every voxel of the union list in one pass.
+// batch re-integration: up to BF_MULTI_MAX_OPS (old pose, new pose, frame) triples applied to every voxel of the union list in one pass; batch
+// integration: (pose, frame) pairs, hpOld NULL in every op (the stencil's kOldPose = false instantiation).
 // work item = {block x, y, z, slot}, its mask = 2 bits per op {old pose may touch the block, new pose may}.  Items are bucketed by cost (number of
 // set bits, quartiles of 2 nOps): quartile 3 at workA[0 ..), quartile 2 at workA[cap - 1 ..] downwards, quartile 1 at workB[0 ..), quartile 0 at
 // workB[cap - 1 ..] downwards (counts in ctrs[set + SET_WORK / SET_Q2 / SET_Q1 / SET_Q0]); the stencil deals them in that order, costliest first.

@@ -58,6 +58,15 @@ class BFFrameLoopFinishInfo(C.Structure):
                 "valid_transforms": self.numValidTransforms, "heap_free": self.heapFreeCount, "valid": bool(self.valid), "done": bool(self.done)}
 
 
+class BFFrameLoopFuseInfo(C.Structure):
+    _fields_ = [("framesFused", C.c_uint32), ("framesSkipped", C.c_uint32), ("batches", C.c_uint32), ("heapFreeCount", C.c_uint32),
+                ("insertsDropped", C.c_ulonglong)]
+
+    def as_dict(self):
+        return {"frames_fused": self.framesFused, "frames_skipped": self.framesSkipped, "batches": self.batches, "heap_free": self.heapFreeCount,
+                "inserts_dropped": int(self.insertsDropped)}
+
+
 class BFFrameLoopGlobalProblem(C.Structure):
     _fields_ = [("d_correspondences", C.c_void_p), ("numCorrespondences", C.c_uint32), ("numKeyframes", C.c_uint32), ("d_validImages", C.c_void_p),
                 ("d_trajectory", C.c_void_p), ("d_cacheFrames", C.c_void_p), ("cacheWidth", C.c_uint32), ("cacheHeight", C.c_uint32),
@@ -88,6 +97,7 @@ def _bind(L):
     L.bfFrameLoopStepPastEnd.argtypes = [vp, C.POINTER(BFFrameLoopStatus)]
     L.bfFrameLoopFinish.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(BFFrameLoopFinishInfo)]
     L.bfFrameLoopGetGlobalProblem.argtypes = [vp, C.POINTER(BFFrameLoopGlobalProblem)]
+    L.bfFrameLoopFuse.argtypes = [vp, C.POINTER(capi.BFHashDataStruct), C.POINTER(BFHashParams), vp, C.c_uint32, C.POINTER(BFFrameLoopFuseInfo)]
     L.bfFrameLoopGetKeyframes.argtypes = [vp, vp]
     L.bfFrameLoopGetTrajectory.argtypes = [vp, vp, C.c_uint]
     L.bfFrameLoopGetTrajectory.restype = C.c_uint
@@ -166,6 +176,25 @@ class FrameLoop:
         rc = self.lib.bfFrameLoopFinish(self._h, int(solve_frames_before_exit), int(max_turns), C.byref(info))
         if rc != CUDA_ERROR_NOT_READY:
             capi.check(rc, "bfFrameLoopFinish")
+        return info.as_dict()
+
+    def fuse(self, scene, poses=None, n: int | None = None) -> dict:
+        """Fuse frames [0, n) of the frame store (default: every frame stepped) into ``scene`` (a CUDASceneRepHashSDF of any voxel size) along
+        ``poses`` [n, 4, 4] camera-to-world (default: the loop's optimised trajectory) -- bfFrameLoopFuse: frames whose pose is not finite are
+        skipped, the others go in batches of <= 16 with a garbage collection after each.  The loop itself does not change.  Returns the info."""
+        self._bind_stream()
+        scene._bind_stream()
+        if n is None:
+            n = self.counters()["frames"]
+        T = None
+        if poses is not None:
+            T = np.ascontiguousarray(poses, dtype=np.float32).reshape(-1, 16)
+            if len(T) < n:
+                raise ValueError(f"{len(T)} poses for {n} frames")
+        info = BFFrameLoopFuseInfo()
+        capi.check(self.lib.bfFrameLoopFuse(self._h, C.byref(scene.m_hashData), C.byref(scene.m_hashParams), None if T is None else T.ctypes.data, int(n),
+                                            C.byref(info)), "bfFrameLoopFuse")
+        scene.m_numIntegratedFrames += info.framesFused
         return info.as_dict()
 
     def global_problem(self) -> BFFrameLoopGlobalProblem:

@@ -4,6 +4,8 @@ trajectory; FL/FriedLiver.cpp, FL/DepthSensing/DepthSensing.cpp:966-1129, 1180-1
 the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every stage is the C-ABI's.
 
     python -m bundlefusion_b200.scan scan.sens out.ply [--frames N] [--device cuda:0] [--solve-frames-before-exit 30]
+        [--mesh-voxel-size V]       after the loop, fuse its frames along the final trajectory into a V-sized hash and mesh that (bundlefusion_b200.fuse)
+        [--poses recorded]          no loop: fuse along the poses stored with the frames (the reference's s_binaryDumpSensorUseTrajectory)
 """
 from __future__ import annotations
 
@@ -14,8 +16,10 @@ import json
 import numpy as np
 
 from . import _capi as capi
+from . import fuse
 from .frame_loop import FrameLoop, default_params
 from .marching_cubes import CUDAMarchingCubesHashSDF, marching_cubes_params
+from .scene_rep import CUDASceneRepHashSDF
 from .sens import SensorDataReader
 
 
@@ -28,20 +32,16 @@ class _LoopScene:
 
 
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
-                sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None) -> dict:
+                sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None,
+                mesh_voxel_size: float | None = None) -> dict:
     """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
     solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
     global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
-    None runs a fixed submapSize + 2 past-end turns."""
+    None runs a fixed submapSize + 2 past-end turns.  mesh_voxel_size=V: the loop's frames are then fused along its final trajectory into a
+    fresh hash of voxel size V (FrameLoop.fuse) and that model is meshed instead of the online one; that call's info goes under "fuse"."""
     r = SensorDataReader(sens_path)
-    hd = r.header
     n = len(r) if max_frames is None else min(len(r), max_frames)
-    P = default_params(hd.depthWidth, hd.depthHeight)
-    P.colorWidth, P.colorHeight = hd.colorWidth, hd.colorHeight          # the ingest resamples colour to the integration size, as CUDAImageManager::process does
-    for k in range(16):
-        P.depthIntrinsics[k] = hd.depthIntrinsic[k]; P.colorIntrinsics[k] = hd.colorIntrinsic[k]
-    P.maxNumFrames = max(32, n + int(P.submapSize))                                  # frame store / trajectories: the sequence plus one chunk of slack
-    P.maxNumImages = max(8, (int(P.maxNumFrames) + int(P.submapSize) - 1) // int(P.submapSize) + 1)      # one keyframe per chunk
+    P = fuse.recording_params(r.header, n)
     if hash_buckets is not None:
         P.hash.m_hashNumBuckets = hash_buckets
     if sdf_blocks is not None:
@@ -69,7 +69,13 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
            "mesh_path": None, "triangles": 0}
     if finish is not None:
         out["finish"] = finish
-    if ply_path is not None:
+    if mesh_voxel_size is not None:
+        scene = CUDASceneRepHashSDF(fuse.fine_hash_params(P, mesh_voxel_size), device)
+        out["fuse"] = loop.fuse(scene, n=n)
+        if ply_path is not None:
+            out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles))
+        scene.close()
+    elif ply_path is not None:
         mp = marching_cubes_params(int(P.hash.m_hashNumBuckets), float(P.hash.m_virtualVoxelSize), max_num_triangles)
         mc = CUDAMarchingCubesHashSDF(mp, device)
         out["triangles"] = mc.extractIsoSurface(_LoopScene(loop)) // 3
@@ -115,13 +121,27 @@ def main(argv=None) -> int:
     ap.add_argument("--solve-frames-before-exit", type=int, default=None, metavar="K",
                     help="end the recording as the reference does: global solves for K turns past the last frame, the dense global solve at turn K, then "
                          "re-integration until every frame is fused at its final pose (the reference's value is 30); without it, a fixed 12 past-end turns")
+    ap.add_argument("--mesh-voxel-size", type=float, default=None, metavar="V",
+                    help="fuse the frames again along the final trajectory into a hash of voxel size V (metres, e.g. 0.004) and mesh that instead of the online model")
+    ap.add_argument("--poses", choices=("recorded",), default=None,
+                    help="'recorded': no bundling -- fuse along the poses stored with the frames (at --mesh-voxel-size, default the loop's 1 cm) and mesh that")
     a = ap.parse_args(argv)
-    o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit)
+    if a.poses == "recorded":
+        voxel = a.mesh_voxel_size if a.mesh_voxel_size is not None else float(default_params(16, 16).hash.m_virtualVoxelSize)
+        o = fuse.fuse_recording(a.sens, a.ply, voxel, "recorded", a.hash_buckets, a.sdf_blocks, a.device, a.frames)
+        o["scene"].close()
+        print(json.dumps({"frames": o["frames"], "fuse": {k: o[k] for k in ("fused", "skipped", "batches", "inserts_dropped", "heap_free")},
+                          "triangles": o["triangles"], "mesh_path": o["mesh_path"]}))
+        return 0
+    o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit,
+                    mesh_voxel_size=a.mesh_voxel_size)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
     summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path")}
     if "finish" in o:
         summary["finish"] = o["finish"]                     # its "valid": StopScanningAndExit's verdict on the reconstruction
+    if "fuse" in o:
+        summary["fuse"] = {k: o["fuse"][k] for k in ("frames_fused", "frames_skipped", "batches", "inserts_dropped", "heap_free")}
     gt = recorded_poses(a.sens, a.frames)
     if np.isfinite(gt).all(axis=(1, 2)).sum() >= 3:
         summary["ate"] = ate(o["trajectory"], gt[:len(o["trajectory"])])

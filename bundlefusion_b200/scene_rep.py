@@ -172,6 +172,22 @@ class CUDASceneRepHashSDF:
                    "bfTsdfIntegrateFrame(deIntegrate)")
         self.m_numIntegratedFrames -= 1
 
+    def integrateBatch(self, frames, poses, depth_ptrs, color_ptrs, cam: BFDepthCameraParams):
+        """n <= 16 integrations in one pass (bfTsdfIntegrateBatch): frame frames[k] of the image arrays at camera-to-world pose poses[k] [n, 4, 4],
+        bit-identical to n integrate() calls in that order.  depth_ptrs / color_ptrs: the frame images as cuda tensors or raw device pointers
+        (indexed by frames[k]).  Asynchronous."""
+        self._bind_stream()
+        f = np.ascontiguousarray(frames, dtype=np.int32).reshape(-1)
+        T = np.ascontiguousarray(poses, dtype=np.float32).reshape(-1, 16)
+        if len(f) != len(T):
+            raise ValueError("frames and poses differ in length")
+        ptr = lambda x: x if isinstance(x, int) or x is None else x.data_ptr()
+        dptr = (C.c_void_p * len(depth_ptrs))(*[ptr(x) for x in depth_ptrs])
+        cptr = (C.c_void_p * len(color_ptrs))(*[ptr(x) for x in color_ptrs])
+        capi.check(self.lib.bfTsdfIntegrateBatch(C.byref(self.m_hashData), C.byref(self.m_hashParams), C.byref(cam), f.ctypes.data, T.ctypes.data, len(f),
+                                                  C.cast(dptr, C.c_void_p), C.cast(cptr, C.c_void_p)), "bfTsdfIntegrateBatch")
+        self.m_numIntegratedFrames += len(f)
+
     def garbageCollect(self):
         """h:110-126 (identify + free over the last compactified list)."""
         self._bind_stream()

@@ -151,6 +151,24 @@ typedef struct BFFrameLoopFinishInfo {
  * the reconstruction stream is joined into the library stream before the call returns. */
 int bfFrameLoopFinish(BFFrameLoop* loop, uint32_t numSolveFramesBeforeExit, uint32_t maxTurns, BFFrameLoopFinishInfo* info);
 
+/* Fusion along a fixed trajectory: frames [0, numFrames) of the loop's frame store, frame f at the camera-to-world pose h_poses[f] (host,
+ * [numFrames][16], row-major; NULL: the loop's optimised trajectory, bfFrameLoopGetTrajectory), integrated with the loop's integration camera
+ * into a caller's voxel hash of any voxel size / truncation (bfTsdfReset it first; it must not be the loop's own).  Frames whose pose is not
+ * finite (the trajectory's invalid frames are all -inf) are skipped.  The others go in order, in batches of <= 16 frames with a garbage
+ * collection after each: one bfTsdfIntegrateBatch + bfTsdfGarbageCollect per batch when batching is usable (fast arithmetic and batching on,
+ * the rule bfTsdfRunOps applies), else the same op list [INTEGRATE x <= 16, GARBAGE_COLLECT] through bfTsdfRunOps.  The reconstruction stream
+ * is joined first; the work is queued on the library stream, and the call synchronises it to fill *info.  Nothing in the loop's own model or
+ * state changes.  On return hashParams holds the last fused pose.  cudaErrorInvalidValue without running anything: NULL loop / hash / params,
+ * an announced look-ahead frame pending (as bfFrameLoopFinish), numFrames beyond the frames stepped, or the loop's own hash. */
+typedef struct BFFrameLoopFuseInfo {
+    uint32_t framesFused;            /* frames integrated */
+    uint32_t framesSkipped;          /* frames whose pose is not finite */
+    uint32_t batches;                /* batches of <= 16 frames, one garbage collection each */
+    uint32_t heapFreeCount;          /* free voxel blocks of the caller's hash at the end */
+    unsigned long long insertsDropped;   /* block inserts dropped since the hash's reset (bfTsdfGetLastFrameStats out[3]): non-zero = heap or table too small */
+} BFFrameLoopFuseInfo;
+int bfFrameLoopFuse(BFFrameLoop* loop, BFHashDataStruct* hashData, BFHashParams* hashParams, const float* h_poses, uint32_t numFrames, BFFrameLoopFuseInfo* info);
+
 /* Test accessor: the global (keyframe) bundle-adjustment problem as the loop holds it -- its own device pointers, valid until the next loop call.
  * The next global solve of the loop runs on exactly these inputs. */
 typedef struct BFFrameLoopGlobalProblem {

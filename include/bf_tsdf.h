@@ -245,6 +245,18 @@ int bfTsdfReintegrateBatch(BFHashDataStruct* hashData, BFHashParams* hashParams,
                            const BFTsdfReintegration* pairs, int numPairs, const float* const* d_depthFrames, const uint8_t* const* d_colorFrames);
 int bfTsdfSetBatching(int enable);
 
+/* n (1..16) integrations of frames[k] at poses[k] (camera-to-world, row-major [n][16]) -- n calls of CUDASceneRepHashSDF::integrate --
+ * as n alloc launches, ONE union list and ONE stencil pass.  Fast arithmetic; bit-identical to n bfTsdfIntegrateFrame calls in the same order
+ * (block set, heap and free list, every voxel word, the live-voxel counters and so what a following bfTsdfGarbageCollect frees), including
+ * frames whose blocks a later frame of the batch inserts (they stay invisible to the earlier frames), frames with no valid pixel and a heap
+ * that runs out inside the batch.  The machinery is bfTsdfReintegrateBatch's (op-tagged allocs, union list, cost buckets, depth-tile cull)
+ * compiled with no old pose: no old frustum is tested and nothing is de-integrated.  On return hashParams holds the last pose and
+ * d_hashCompactified the union list (its GC flags mark the last frame's frustum).  Returns cudaErrorInvalidValue with nothing enqueued for
+ * n < 1 or n > 16, NULL frames / poses / frame arrays, a negative frame index or one whose depth or colour pointer is NULL.  In exact
+ * arithmetic (bfTsdfSetArithmetic) it runs the fast pass, as bfTsdfReintegrateBatch does. */
+int bfTsdfIntegrateBatch(BFHashDataStruct* hashData, BFHashParams* hashParams, const BFDepthCameraParams* depthCameraParams,
+                         const int32_t* frames, const float* poses, int n, const float* const* d_depthFrames, const uint8_t* const* d_colorFrames);
+
 /* CUDASceneRepHashSDF::garbageCollect (h:110-126) over the last compactified list */
 int bfTsdfGarbageCollect(BFHashDataStruct* hashData, const BFHashParams* hashParams);
 
