@@ -90,6 +90,10 @@ class BFHashDataStruct(C.Structure):
     ]
 
 
+class BFBlockKeySet(C.Structure):
+    _fields_ = [("d_keys", C.c_void_p), ("d_counters", C.c_void_p), ("capacity", C.c_uint32)]
+
+
 assert C.sizeof(BFHashParams) == 224, C.sizeof(BFHashParams)
 assert BFHashParams.m_dummy.offset == 216
 assert C.sizeof(BFHashEntry) == 32 and C.sizeof(BFVoxel) == 12
@@ -104,7 +108,7 @@ TSDF_SYMBOLS = [
     "bfSetStream", "bfGetStream", "bfGetLastErrorString", "bfTsdfAuxBytes", "bfTsdfReset", "bfTsdfIntegrateFrame",
     "bfTsdfGarbageCollect", "bfTsdfGetHeapFreeCount", "bfTsdfGetNumOccupiedBlocks", "bfTsdfGetLastFrameStats",
     "bfTsdfReleaseAux", "bfTsdfReintegrateFrame", "bfGetLaunchCount", "bfTsdfSetProfiling", "bfTsdfGetProfile", "bfTsdfGetProfileEx", "bfTsdfSetLanes", "bfTsdfSetArithmetic", "bfTsdfReintegrateBatch", "bfTsdfSetBatching",
-    "bfTsdfIntegrateBatch",
+    "bfTsdfIntegrateBatch", "bfTsdfCountBlocks", "bfTsdfBlockKeyLoad", "bfTsdfBlockKeyMerge",
 ]
 
 HOST_SYMBOLS = ["bfMat4Inverse", "bfTsdfRunOps"]
@@ -316,6 +320,9 @@ def lib() -> C.CDLL:
     L.bfMat4Inverse.restype = None
     L.bfTsdfRunOps.argtypes = [P(BFHashDataStruct), P(BFHashParams), P(BFDepthCameraParams), P(BFTsdfOp), C.c_int, P(vp), P(vp)]
     L.bfTsdfIntegrateBatch.argtypes = [P(BFHashDataStruct), P(BFHashParams), P(BFDepthCameraParams), vp, vp, C.c_int, vp, vp]
+    L.bfTsdfCountBlocks.argtypes = [P(BFBlockKeySet), P(BFHashParams), P(BFDepthCameraParams), vp, vp, C.c_int, vp]
+    L.bfTsdfBlockKeyLoad.argtypes = [P(BFBlockKeySet), C.c_uint32, vp, vp]
+    L.bfTsdfBlockKeyMerge.argtypes = [P(BFBlockKeySet), P(BFBlockKeySet)]
     # solver
     L.solveBundlingStub.argtypes = [P(BFSolverInput), P(BFSolverState), P(BFSolverParameters), P(BFSolverStateAnalysis), P(C.c_float), vp]
     L.solveBundlingStub.restype = None

@@ -26,6 +26,7 @@
 #include "../../include/bf_tsdf.h"
 #include "bf_common.cuh"
 #include "tsdf_shared.cuh"
+#include "tsdf_keys.cuh"
 #include "mat4.cuh"
 
 namespace bf {
@@ -95,7 +96,6 @@ static int get_aux(const BFHashDataStruct* hd, const BFHashParams* hp, TsdfAux**
 // device math shared by every kernel (bit-exact mirror of oracle/tsdf_oracle.c)
 // ------------------------------------------------------------------------------------------
 struct F3 { float x, y, z; };
-struct I3 { int x, y, z; };
 
 __device__ __forceinline__ int isign(float v) { return (0.0f < v) - (v < 0.0f); }
 
@@ -107,11 +107,6 @@ __device__ __forceinline__ F3 xform(const BFFloat4x4& M, F3 v) {
     r.y = __fmaf_rn(v.z, M.m[6], __fmaf_rn(v.x, M.m[4], v.y * M.m[5])) + M.m[7];
     r.z = __fmaf_rn(v.z, M.m[10], __fmaf_rn(v.x, M.m[8], v.y * M.m[9])) + M.m[11];
     return r;
-}
-// VoxelUtilHashSDF.h:226-234 (unsigned modulo, see oracle note)
-__device__ __forceinline__ unsigned hash_pos(unsigned numBuckets, I3 p) {
-    unsigned v = ((unsigned)p.x * 73856093u) ^ ((unsigned)p.y * 19349669u) ^ ((unsigned)p.z * 83492791u);
-    return v % numBuckets;
 }
 __device__ __forceinline__ float truncation(const BFHashParams& hp, float z) { return __fmaf_rn(hp.m_truncScale, z, hp.m_truncation); }
 __device__ __forceinline__ I3 world_to_voxel(const BFHashParams& hp, F3 pos) {
@@ -405,11 +400,6 @@ __device__ __forceinline__ bool block_can_pass_m(float s, float T, float vs, con
     if (!(dmax >= dmin)) return false;                      // no acceptable depth under the footprint
     return !(zmin >= dmax * (1.0f + s) + T + eps || zmax <= dmin * (1.0f - s) - T - eps);
 }
-__device__ __forceinline__ I3 unpack_block_key(unsigned long long key) {
-    const int lim = 1 << 20;
-    I3 b = { (int)((key >> 42) & 0x1FFFFF) - lim, (int)((key >> 21) & 0x1FFFFF) - lim, (int)(key & 0x1FFFFF) - lim };
-    return b;
-}
 
 // Multi-GPU spatial shard (SURVEY.md section 8e): when hp.m_dummy = {rank, world} with world > 1, this device allocates
 // (and therefore integrates) only the blocks it owns.  Ownership is a 3-D checkerboard of cubes of BF_SHARD_CUBE^3 blocks
@@ -501,22 +491,60 @@ __device__ __forceinline__ bool dda_step(DDA& s, int& axis) {
     else         { s.cur.y = v; s.tMax.y += s.tDelta.y; axis = 1; }
     return true;
 }
-// the reference's single-phase walk: every visited in-frustum block goes straight to the table (rare fallback)
-__device__ __noinline__ void alloc_pixel_direct(const BFHashDataStruct& hd, const BFHashParams& hp, const BFDepthCameraParams& cp,
-                                                const float* __restrict__ depth, unsigned x, unsigned y, int4* slotInfo, unsigned* ctrs, AllocEpoch ep) {
+// Where the alloc walk hands each block it would insert (in frustum, owned by this rank): a compile-time sink, which receives the walk's
+// trailing arguments.  AllocSink inserts the block into the voxel hash (the alloc launches of every integrate path); KeySetSink records its key
+// in a caller's key set (bfTsdfCountBlocks), so the counted union is the set of blocks the alloc launches would insert, by construction.
+// direct() runs the sink's single-phase walk of one pixel.
+struct AllocSink {
+    __device__ static __forceinline__ void put(const BFHashParams& hp, I3 b, const BFHashDataStruct* hd, int4* slotInfo, unsigned* ctrs, AllocEpoch ep) {
+        alloc_block(*hd, hp, slotInfo, ctrs, b, ep);
+    }
+    __device__ static __forceinline__ void direct(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned x, unsigned y,
+                                                  const BFHashDataStruct* hd, int4* slotInfo, unsigned* ctrs, AllocEpoch ep);
+};
+struct KeySetSink {
+    __device__ static __forceinline__ void put(const BFHashParams&, I3 b, unsigned long long* keys, unsigned mask, unsigned* keyCtrs) {
+        keyset_insert_block(keys, mask, keyCtrs, b);
+    }
+    __device__ static __forceinline__ void direct(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned x, unsigned y,
+                                                  unsigned long long* keys, unsigned mask, unsigned* keyCtrs);
+};
+
+// the reference's single-phase walk: every visited in-frustum block goes straight to the sink (rare fallback)
+template <class Sink, class... A>
+__device__ __forceinline__ void walk_pixel_direct(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned x, unsigned y,
+                                                  A... args) {
     DDA s;
     if (!dda_setup(hp, cp, depth, x, y, s)) return;
 #pragma unroll 1
     for (unsigned iter = 0; iter < 1024; ++iter) {
-        if (block_in_frustum(hp, cp, s.cur) && owns_block(hp, s.cur)) alloc_block(hd, hp, slotInfo, ctrs, s.cur, ep);
+        if (block_in_frustum(hp, cp, s.cur) && owns_block(hp, s.cur)) Sink::put(hp, s.cur, args...);
         int axis;
         if (!dda_step(s, axis)) return;
     }
 }
+__device__ __noinline__ void alloc_pixel_direct(const BFHashDataStruct& hd, const BFHashParams& hp, const BFDepthCameraParams& cp,
+                                                const float* __restrict__ depth, unsigned x, unsigned y, int4* slotInfo, unsigned* ctrs, AllocEpoch ep) {
+    walk_pixel_direct<AllocSink>(hp, cp, depth, x, y, &hd, slotInfo, ctrs, ep);
+}
+__device__ __noinline__ void count_pixel_direct(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned x, unsigned y,
+                                                unsigned long long* keys, unsigned mask, unsigned* keyCtrs) {
+    walk_pixel_direct<KeySetSink>(hp, cp, depth, x, y, keys, mask, keyCtrs);
+}
+__device__ __forceinline__ void AllocSink::direct(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned x, unsigned y,
+                                                  const BFHashDataStruct* hd, int4* slotInfo, unsigned* ctrs, AllocEpoch ep) {
+    alloc_pixel_direct(*hd, hp, cp, depth, x, y, slotInfo, ctrs, ep);
+}
+__device__ __forceinline__ void KeySetSink::direct(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned x, unsigned y,
+                                                   unsigned long long* keys, unsigned mask, unsigned* keyCtrs) {
+    count_pixel_direct(hp, cp, depth, x, y, keys, mask, keyCtrs);
+}
 
-__global__ void __launch_bounds__(256, 8)    // 32 regs: the whole 640x480 frame is resident in one wave
-alloc_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp,
-             const float* __restrict__ depth, int4* slotInfo, unsigned* ctrs, float2* tiles, int zeroSet, AllocEpoch ep) {
+// The body of the alloc launch over one 16x16 tile (see above).  ctrs / zeroSet / tiles: alloc_kernel's counter-set zeroing and depth tiles
+// (nullptr / -1 / nullptr when counting).
+template <class Sink, class... A>
+__device__ __forceinline__ void alloc_walk(const BFHashParams& hp, const BFDepthCameraParams& cp, const float* __restrict__ depth, unsigned* ctrs, float2* tiles,
+                                           int zeroSet, A... args) {
     __shared__ unsigned long long sSet[BF_ALLOC_SET];
     __shared__ float2 sRed[8];
     const unsigned tid = threadIdx.y * blockDim.x + threadIdx.x;
@@ -578,9 +606,22 @@ alloc_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const
         const unsigned long long key = sSet[i];
         if (key == 0ull) continue;
         const I3 b = unpack_block_key(key);
-        if (block_in_frustum(hp, cp, b) && owns_block(hp, b)) alloc_block(hd, hp, slotInfo, ctrs, b, ep);
+        if (block_in_frustum(hp, cp, b) && owns_block(hp, b)) Sink::put(hp, b, args...);
     }
-    if (needDirect) alloc_pixel_direct(hd, hp, cp, depth, x, y, slotInfo, ctrs, ep);   // set overflow / coordinates out of key range
+    if (needDirect) Sink::direct(hp, cp, depth, x, y, args...);   // set overflow / coordinates out of key range
+}
+
+__global__ void __launch_bounds__(256, 8)    // 32 regs: the whole 640x480 frame is resident in one wave
+alloc_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp,
+             const float* __restrict__ depth, int4* slotInfo, unsigned* ctrs, float2* tiles, int zeroSet, AllocEpoch ep) {
+    alloc_walk<AllocSink>(hp, cp, depth, ctrs, tiles, zeroSet, &hd, slotInfo, ctrs, ep);
+}
+
+// bfTsdfCountBlocks: the same walk, every block into the key set instead of the hash
+__global__ void __launch_bounds__(256, 8)
+count_blocks_kernel(const __grid_constant__ BFHashParams hp, const __grid_constant__ BFDepthCameraParams cp, const float* __restrict__ depth,
+                    unsigned long long* keys, unsigned mask, unsigned* keyCtrs) {
+    alloc_walk<KeySetSink>(hp, cp, depth, nullptr, nullptr, -1, keys, mask, keyCtrs);
 }
 
 // compactify: list of allocated AND in-frustum blocks (CUDASceneRepHashSDF.cu:324-366),
@@ -1521,6 +1562,52 @@ BF_API int bfTsdfIntegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const BF
     return run_batch(hd, hp, cp, n, frames, oldPoses, newPoses, d_depthFrames, d_colorFrames);
 }
 namespace bf { int tsdf_batching_usable() { return (batching_on() && arith_fast()) ? 1 : 0; } }
+
+static bool key_set_ok(const BFBlockKeySet* set) {
+    return set && set->d_keys && set->d_counters && set->capacity != 0 && (set->capacity & (set->capacity - 1)) == 0 && set->capacity <= (1u << 31);
+}
+
+// the alloc launches of bfTsdfIntegrateBatch, each block into the key set instead of the hash: per frame the parameters run_batch forms (the pose
+// and its host inverse, mat4_inverse_ref), the same grid
+BF_API int bfTsdfCountBlocks(BFBlockKeySet* set, const BFHashParams* hp, const BFDepthCameraParams* cp, const int32_t* frames, const float* poses, int n,
+                             const float* const* d_depthFrames) {
+    if (n < 1 || n > BF_MULTI_MAX_OPS || !key_set_ok(set) || !hp || !cp || !frames || !poses || !d_depthFrames) return (int)cudaErrorInvalidValue;
+    for (int k = 0; k < n; ++k)
+        if (frames[k] < 0 || !d_depthFrames[frames[k]]) return (int)cudaErrorInvalidValue;
+    dim3 block(BF_TILE, BF_TILE);
+    dim3 grid((cp->m_imageWidth + block.x - 1) / block.x, (cp->m_imageHeight + block.y - 1) / block.y);
+    for (int k = 0; k < n; ++k) {
+        BFHashParams q = *hp;
+        for (int e = 0; e < 16; ++e) q.m_rigidTransform.m[e] = poses[16 * (size_t)k + e];
+        mat4_inverse_ref(poses + 16 * (size_t)k, q.m_rigidTransformInverse.m);
+        ++g_launchCount;
+        count_blocks_kernel<<<grid, block, 0, g_stream>>>(q, *cp, d_depthFrames[frames[k]], reinterpret_cast<unsigned long long*>(set->d_keys), set->capacity - 1u,
+                                                          set->d_counters);
+        BF_CHECK(cudaGetLastError());
+    }
+    return 0;
+}
+
+BF_API int bfTsdfBlockKeyLoad(const BFBlockKeySet* set, uint32_t numBuckets, uint32_t* d_bucketLoad, uint32_t* d_out) {
+    if (!key_set_ok(set) || numBuckets == 0 || !d_bucketLoad || !d_out) return (int)cudaErrorInvalidValue;
+    BF_CHECK(cudaMemsetAsync(d_bucketLoad, 0, sizeof(uint32_t) * (size_t)numBuckets, g_stream));
+    BF_CHECK(cudaMemsetAsync(d_out, 0, sizeof(uint32_t) * 3, g_stream));
+    ++g_launchCount;
+    bucket_load_kernel<<<grid_for((set->capacity + 255) / 256, 2), 256, 0, g_stream>>>(reinterpret_cast<const unsigned long long*>(set->d_keys), set->capacity,
+                                                                                       numBuckets, d_bucketLoad, d_out);
+    BF_CHECK(cudaGetLastError());
+    return 0;
+}
+
+BF_API int bfTsdfBlockKeyMerge(BFBlockKeySet* dst, const BFBlockKeySet* src) {
+    if (!key_set_ok(dst) || !key_set_ok(src) || dst->d_keys == src->d_keys) return (int)cudaErrorInvalidValue;
+    ++g_launchCount;
+    keyset_merge_kernel<<<grid_for((src->capacity + 255) / 256, 4), 256, 0, g_stream>>>(reinterpret_cast<unsigned long long*>(dst->d_keys), dst->capacity - 1u,
+                                                                                        dst->d_counters, reinterpret_cast<const unsigned long long*>(src->d_keys),
+                                                                                        src->capacity);
+    BF_CHECK(cudaGetLastError());
+    return 0;
+}
 
 BF_API int bfTsdfGarbageCollect(BFHashDataStruct* hd, const BFHashParams* hp) {
     TsdfAux* aux;

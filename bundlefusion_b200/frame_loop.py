@@ -197,6 +197,36 @@ class FrameLoop:
         scene.m_numIntegratedFrames += info.framesFused
         return info.as_dict()
 
+    def fit_hash_params(self, voxel_size: float, poses=None, n: int | None = None, max_table_bytes: int | None = None):
+        """Hash parameters for fuse() of frames [0, n) (default: every frame stepped) along ``poses`` (default: the optimised trajectory) at
+        voxel_size, sized from a count of the blocks that fusion will allocate (fuse.BlockCounter over the frame store; frames whose pose is not
+        finite are skipped, as fuse() skips them): the loop's hash parameters at voxel_size with the heap and bucket count fuse.fit_hash_params
+        picks.  The loop itself does not change.  Returns (BFHashParams, report)."""
+        from . import fuse
+        self.join()
+        if n is None:
+            n = self.counters()["frames"]
+        if poses is None:
+            T = np.full((n, 16), -np.inf, np.float32)
+            traj = self.trajectory(n).reshape(-1, 16)
+            T[:len(traj)] = traj
+        else:
+            T = np.ascontiguousarray(poses, dtype=np.float32).reshape(-1, 16)
+            if len(T) < n:
+                raise ValueError(f"{len(T)} poses for {n} frames")
+        fin = [f for f in range(n) if np.isfinite(T[f]).all()]
+        hp = BFHashParams()
+        C.memmove(C.byref(hp), C.byref(self.params.hash), C.sizeof(BFHashParams))
+        hp.m_virtualVoxelSize = voxel_size
+        counter = fuse.BlockCounter(hp, self.device)
+        depth = []
+        for f in fin:
+            d, c = C.c_void_p(), C.c_void_p()
+            capi.check(self.lib.bfFrameLoopGetFrame(self._h, int(f), C.byref(d), C.byref(c)), "bfFrameLoopGetFrame")
+            depth.append(d.value)
+        counter.add(depth, T[fin], fuse.integration_camera(self.params))
+        return fuse.fit_hash_params(self.params.hash, voxel_size, counter, max_table_bytes)
+
     def global_problem(self) -> BFFrameLoopGlobalProblem:
         """the keyframe bundle-adjustment problem as the loop holds it (its device pointers, valid until the next loop call)"""
         out = BFFrameLoopGlobalProblem()

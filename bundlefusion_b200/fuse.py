@@ -5,6 +5,12 @@ finer voxel size (4-5 mm) and mesh that.
 
     fuse_recording(sens_path, ply_path, voxel_size=0.004, poses="recorded")      # a .sens file along its own poses
     FrameLoop.fuse(scene, poses=None)                                              # the loop's frame store along its optimised trajectory
+    fuse_recording(..., fit_hash=True)                                             # the hash sized from a count of the blocks it will hold
+
+Sizing: BlockCounter counts on the device the union of the blocks the fusion's alloc launches will insert (bfTsdfCountBlocks), and
+fit_hash_params sizes the hash from it -- a heap of exactly that many blocks and the fewest buckets (of a fixed sequence) in which no bucket
+receives more than BF_HASH_BUCKET_SIZE of them.  The blocks live in the fused hash are always a subset of that union, so such a hash never
+drops an insert and its heap never runs out (include/bf_tsdf.h).
 
 Host glue only: each frame is decoded (the next one while the device works), ingested exactly as the frame loop ingests it (bfIngestFrame) into
 a ring of 16 device slots, and every 16 frames with a finite pose go into the hash in one bfTsdfIntegrateBatch pass, with a garbage collection
@@ -22,6 +28,14 @@ from .scene_rep import CUDASceneRepHashSDF
 from .sens import SensorDataReader
 
 BATCH = 16                       # bfTsdfIntegrateBatch's limit
+# the bytes per bucket CUDASceneRepHashSDF allocates: the hash and compactified entries, the decision and prefix ints, one mutex int
+TABLE_BYTES_PER_BUCKET = capi.BF_HASH_BUCKET_SIZE * (2 * C.sizeof(capi.BFHashEntry) + 2 * 4) + 4
+BUCKET_GROWTH = 1.25             # ratio of fit_hash_params' bucket-count sequence
+MAX_BUCKETS = (2 ** 32 - 1) // capi.BF_HASH_BUCKET_SIZE        # entry indices are 32-bit in the kernels
+# fit_hash_params' bucket cap when no max_table_bytes is given.  The reference's bucket function maps many distinct blocks to the same 32-bit
+# value, so on large scans no bucket count removes every overflow (a 1.4 M-block surface keeps 32 blocks over at any count; an 800 k-block
+# box needs more than 55 buckets per block); the cap keeps the table finite and the fit reports what remains as "predicted_overflow".
+DEFAULT_BUCKETS_PER_BLOCK = 32
 
 
 def recording_params(header, n: int):
@@ -70,6 +84,155 @@ def fine_hash_params(P, voxel_size: float, hash_buckets: int | None = None, sdf_
     return hp
 
 
+def table_bytes(buckets: int) -> int:
+    """device bytes of a hash table of `buckets` buckets, as CUDASceneRepHashSDF allocates it (the heap and voxel blocks not included)"""
+    return int(buckets) * TABLE_BYTES_PER_BUCKET
+
+
+def bucket_candidates(count: int, max_buckets: int = MAX_BUCKETS):
+    """the odd bucket counts fit_hash_params tries, in order: floor(max(count, 1) * BUCKET_GROWTH^k) | 1 for k = 0, 1, ..., repeats dropped,
+    up to max_buckets"""
+    base, k, last = max(int(count), 1), 0, 0
+    while True:
+        b = int(base * BUCKET_GROWTH ** k) | 1
+        k += 1
+        if b > max_buckets:
+            return
+        if b > last:
+            last = b
+            yield b
+
+
+class BlockCounter:
+    """The union of the SDF blocks that bfTsdfIntegrateBatch's alloc launches would insert for the frames given to add(), kept on the device
+    (bfTsdfCountBlocks into a BFBlockKeySet in torch storage).  hash_params: the fusion's parameters -- voxel size, truncation,
+    m_maxIntegrationDistance and the m_dummy shard setting; its table sizes are not read.  The set grows by itself: add() merges it into one
+    twice as large, and counts the frames again, whenever a key was refused or the set is more than half full."""
+
+    def __init__(self, hash_params, device="cuda:0", capacity: int = 1 << 16):
+        import torch
+        if capacity < 1 or capacity & (capacity - 1) or capacity > 1 << 31:
+            raise ValueError("capacity: a power of two <= 2^31")
+        self._torch = torch
+        self.device = torch.device(device)
+        self.lib = capi.lib()
+        self.hash_params = capi.BFHashParams()
+        C.memmove(C.byref(self.hash_params), C.byref(hash_params), C.sizeof(capi.BFHashParams))
+        self._set, self._keys, self._ctrs = self._new(capacity)
+        self._load, self._out = None, torch.zeros(3, dtype=torch.int32, device=self.device)
+
+    def _new(self, capacity: int):
+        t = self._torch
+        keys = t.zeros(capacity, dtype=t.int64, device=self.device)
+        ctrs = t.zeros(3, dtype=t.int32, device=self.device)
+        s = capi.BFBlockKeySet()
+        s.d_keys, s.d_counters, s.capacity = keys.data_ptr(), ctrs.data_ptr(), capacity
+        return s, keys, ctrs
+
+    def _bind_stream(self):
+        t = self._torch
+        t.cuda.set_device(self.device)
+        self.lib.bfSetStream(C.c_void_p(t.cuda.current_stream(self.device).cuda_stream))
+
+    def _counters(self):
+        stored, refused, out_of_range = (int(x) for x in self._ctrs.cpu().tolist())
+        if out_of_range:
+            raise RuntimeError(f"{out_of_range} blocks lie more than 2^20 blocks from the origin: the key set cannot hold them")
+        return stored, refused
+
+    def _grow(self, need: int):
+        cap = self._set.capacity
+        while cap < 2 * need:
+            cap *= 2
+        if cap > 1 << 31:
+            raise RuntimeError(f"{need} blocks: more than the key set's 2^30")
+        s, keys, ctrs = self._new(cap)
+        capi.check(self.lib.bfTsdfBlockKeyMerge(C.byref(s), C.byref(self._set)), "bfTsdfBlockKeyMerge")
+        self._set, self._keys, self._ctrs = s, keys, ctrs
+
+    @property
+    def capacity(self) -> int:
+        return int(self._set.capacity)
+
+    def add(self, depth_ptrs, poses, cam, frames=None) -> None:
+        """counts frame frames[k] of depth_ptrs (cuda tensors or raw device pointers; default frames = 0..n-1) at camera-to-world pose poses[k]
+        [n, 4, 4]; any n.  Synchronises once per 16 frames."""
+        T = np.ascontiguousarray(poses, dtype=np.float32).reshape(-1, 16)
+        f = np.arange(len(T), dtype=np.int32) if frames is None else np.ascontiguousarray(frames, dtype=np.int32).reshape(-1)
+        if len(f) != len(T):
+            raise ValueError("frames and poses differ in length")
+        ptr = lambda x: x if isinstance(x, int) or x is None else x.data_ptr()
+        dptr = (C.c_void_p * len(depth_ptrs))(*[ptr(x) for x in depth_ptrs])
+        self._bind_stream()
+        for s in range(0, len(f), BATCH):
+            fk, Tk = f[s:s + BATCH].copy(), T[s:s + BATCH].copy()
+            while True:
+                capi.check(self.lib.bfTsdfCountBlocks(C.byref(self._set), C.byref(self.hash_params), C.byref(cam), fk.ctypes.data, Tk.ctypes.data, len(fk),
+                                                      C.cast(dptr, C.c_void_p)), "bfTsdfCountBlocks")
+                stored, refused = self._counters()
+                if refused or 2 * stored > self.capacity:
+                    self._grow(stored + refused)
+                if not refused:
+                    break
+
+    @property
+    def count(self) -> int:
+        """distinct blocks counted so far (synchronises)"""
+        return self._counters()[0]
+
+    def bucket_load(self, buckets: int) -> dict:
+        """{"keys", "max_load", "over"} of the counted blocks in `buckets` buckets of the hash's bucket function (bfTsdfBlockKeyLoad); over = sum
+        over buckets of max(0, load - BF_HASH_BUCKET_SIZE).  Synchronises."""
+        t = self._torch
+        if self._load is None or self._load.numel() < buckets:
+            self._load = t.empty(int(buckets), dtype=t.int32, device=self.device)
+        self._bind_stream()
+        capi.check(self.lib.bfTsdfBlockKeyLoad(C.byref(self._set), int(buckets), self._load.data_ptr(), self._out.data_ptr()), "bfTsdfBlockKeyLoad")
+        keys, mx, over = (int(x) for x in self._out.cpu().tolist())
+        return {"keys": keys, "max_load": mx, "over": over}
+
+    def keys(self) -> np.ndarray:
+        """the counted block positions, int32 [count, 3], in lexicographic order"""
+        k = self._keys.cpu().numpy().view(np.uint64)
+        k = np.sort(k[k != 0])
+        lim = 1 << 20
+        pos = np.stack([(k >> np.uint64(42)) & np.uint64(0x1FFFFF), (k >> np.uint64(21)) & np.uint64(0x1FFFFF), k & np.uint64(0x1FFFFF)], axis=1)
+        return (pos.astype(np.int64) - lim).astype(np.int32)
+
+
+def fit_hash_params(base_hp, voxel_size: float, counter, max_table_bytes: int | None = None):
+    """Hash parameters for a fusion of the blocks `counter` (a BlockCounter) counted: base_hp's parameters at voxel_size, a heap of exactly the
+    count, and the first bucket count of bucket_candidates(count) under which no bucket holds more than BF_HASH_BUCKET_SIZE counted blocks
+    (over == 0: no insert of the fusion can be dropped).  When no such bucket count fits in max_table_bytes (table_bytes; default: the table of
+    DEFAULT_BUCKETS_PER_BLOCK buckets per counted block), the largest odd one that fits is taken and its over reported as "predicted_overflow".
+    Returns (BFHashParams, report)."""
+    if np.float32(voxel_size) != np.float32(counter.hash_params.m_virtualVoxelSize):
+        raise ValueError(f"the counter counted {counter.hash_params.m_virtualVoxelSize} m voxels, not {voxel_size} m")
+    count = counter.count
+    if max_table_bytes is None:
+        max_table_bytes = table_bytes(DEFAULT_BUCKETS_PER_BLOCK * max(count, 1) + 1)
+    cap = min(MAX_BUCKETS, int(max_table_bytes) // TABLE_BYTES_PER_BUCKET)
+    if cap < 1:
+        raise ValueError(f"max_table_bytes {max_table_bytes}: less than one bucket ({TABLE_BYTES_PER_BUCKET} bytes)")
+    buckets, load, tried = None, None, 0
+    for b in bucket_candidates(count, cap):
+        load, tried = counter.bucket_load(b), tried + 1
+        if load["over"] == 0:
+            buckets = b
+            break
+    if buckets is None:
+        buckets = cap if cap & 1 else cap - 1
+        load, tried = counter.bucket_load(buckets), tried + 1
+    hp = capi.BFHashParams()
+    C.memmove(C.byref(hp), C.byref(base_hp), C.sizeof(capi.BFHashParams))
+    hp.m_virtualVoxelSize = voxel_size
+    hp.m_hashNumBuckets = buckets
+    hp.m_numSDFBlocks = max(1, count)
+    report = {"blocks_counted": count, "buckets": buckets, "sdf_blocks": int(hp.m_numSDFBlocks), "table_bytes": table_bytes(buckets),
+              "max_load": load["max_load"], "predicted_overflow": load["over"], "candidates_tried": tried}
+    return hp, report
+
+
 def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6_000_000) -> dict:
     """iso-surface of a scene (threshold 10 x voxel, the reference's s_SDFMarchingCubeThreshFactor) saved as PLY"""
     hp = scene.m_hashParams
@@ -83,12 +246,18 @@ def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6
 
 def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: float = 0.004, poses="recorded", hash_buckets: int | None = None,
                    sdf_blocks: int | None = None, device="cuda:0", max_frames: int | None = None, scene: CUDASceneRepHashSDF | None = None,
-                   max_num_triangles: int = 6_000_000) -> dict:
+                   max_num_triangles: int = 6_000_000, fit_hash: bool = False, max_table_bytes: int | None = None) -> dict:
     """Fuses a .sens recording along fixed camera-to-world poses -- "recorded" (the poses stored with the frames) or an array [n, 4, 4] --
     into a voxel hash of voxel_size (or into ``scene``, a reset CUDASceneRepHashSDF), with no bundling.  Frames whose pose is not finite are
-    skipped.  Returns {"frames", "fused", "skipped", "batches", "inserts_dropped" (block inserts the hash had no room for: size it up when
-    non-zero), "heap_free", "triangles", "mesh_path", "scene"}."""
+    skipped.  Returns {"frames", "fused", "skipped", "batches", "inserts_dropped" (block inserts the hash had no room for), "heap_free",
+    "triangles", "mesh_path", "scene"}.
+    fit_hash=True sizes the hash from the blocks the fusion will allocate: a first pass decodes and ingests every frame as the fusion does and
+    counts them (BlockCounter), fit_hash_params sizes the hash (within max_table_bytes), and the fusion runs as a second pass.  The result then
+    also holds "blocks_counted", "buckets", "predicted_overflow" (0 unless max_table_bytes was too small to avoid overflow) and the whole
+    report under "fit".  fit_hash excludes hash_buckets, sdf_blocks and scene."""
     import torch
+    if fit_hash and (hash_buckets is not None or sdf_blocks is not None or scene is not None):
+        raise ValueError("fit_hash sizes the hash itself: pass no hash_buckets, sdf_blocks or scene")
     dev = torch.device(device)
     r = SensorDataReader(sens_path)
     try:
@@ -102,8 +271,6 @@ def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: floa
             T = np.ascontiguousarray(poses, np.float32).reshape(-1, 4, 4)
             if len(T) < n:
                 raise ValueError(f"{len(T)} poses for {n} frames")
-        if scene is None:
-            scene = CUDASceneRepHashSDF(fine_hash_params(P, voxel_size, hash_buckets, sdf_blocks), dev)
         cam, ip, lib = integration_camera(P), ingest_params(P), capi.lib()
         Wi, Hi = int(P.integrationWidth), int(P.integrationHeight)
         raw_d = torch.empty((int(P.depthHeight), int(P.depthWidth)), dtype=torch.float32, device=dev)
@@ -112,23 +279,40 @@ def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: floa
         ring_c = torch.empty((BATCH, Hi, Wi, 4), dtype=torch.uint8, device=dev)
         dptr, cptr = [ring_d[k] for k in range(BATCH)], [ring_c[k] for k in range(BATCH)]
         todo = [i for i in range(n) if np.isfinite(T[i]).all()]
+
+        def batches(bind_stream):
+            """decodes and ingests the frames of `todo` into the ring; yields the recording's frame indices of each full ring (or the last)"""
+            cur = r.frame(todo[0], pinned=True) if todo else None
+            for j, i in enumerate(todo):
+                nxt = r.frame(todo[j + 1], pinned=True) if j + 1 < len(todo) else None        # decode the next frame while the device works on this one
+                bind_stream()
+                raw_d.copy_(cur[0], non_blocking=True); raw_c.copy_(cur[1], non_blocking=True)
+                k = j % BATCH
+                capi.check(lib.bfIngestFrame(C.byref(ip), raw_d.data_ptr(), raw_c.data_ptr(), ring_d[k].data_ptr(), ring_c[k].data_ptr()), "bfIngestFrame")
+                if k == BATCH - 1 or j + 1 == len(todo):
+                    yield todo[j - k:j + 1]
+                cur = nxt
+
+        fit = None
+        if fit_hash:
+            counter = BlockCounter(fine_hash_params(P, voxel_size), dev)
+            for idx in batches(counter._bind_stream):
+                counter.add(dptr[:len(idx)], T[idx], cam)
+            hp, fit = fit_hash_params(P.hash, voxel_size, counter, max_table_bytes)
+            del counter
+            scene = CUDASceneRepHashSDF(hp, dev)
+        elif scene is None:
+            scene = CUDASceneRepHashSDF(fine_hash_params(P, voxel_size, hash_buckets, sdf_blocks), dev)
         out = {"frames": n, "fused": len(todo), "skipped": n - len(todo), "batches": 0}
-        cur = r.frame(todo[0], pinned=True) if todo else None
-        for j, i in enumerate(todo):
-            nxt = r.frame(todo[j + 1], pinned=True) if j + 1 < len(todo) else None        # decode the next frame while the device works on this one
-            scene._bind_stream()
-            raw_d.copy_(cur[0], non_blocking=True); raw_c.copy_(cur[1], non_blocking=True)
-            k = j % BATCH
-            capi.check(lib.bfIngestFrame(C.byref(ip), raw_d.data_ptr(), raw_c.data_ptr(), ring_d[k].data_ptr(), ring_c[k].data_ptr()), "bfIngestFrame")
-            if k == BATCH - 1 or j + 1 == len(todo):
-                idx = todo[j - k:j + 1]
-                scene.integrateBatch(np.arange(k + 1), T[idx], dptr, cptr, cam)
-                scene.garbageCollect()
-                out["batches"] += 1
-            cur = nxt
+        for idx in batches(scene._bind_stream):
+            scene.integrateBatch(np.arange(len(idx)), T[idx], dptr, cptr, cam)
+            scene.garbageCollect()
+            out["batches"] += 1
         torch.cuda.synchronize(dev)
         out["inserts_dropped"] = scene.getLastFrameStats()["dropped"] if out["batches"] else 0
         out["heap_free"] = scene.getHeapFreeCount()
+        if fit is not None:
+            out.update(blocks_counted=fit["blocks_counted"], buckets=fit["buckets"], predicted_overflow=fit["predicted_overflow"], fit=fit)
         out.update(triangles=0, mesh_path=None, scene=scene)
         if ply_path is not None:
             out.update(mesh_scene(scene, ply_path, device, max_num_triangles))

@@ -6,6 +6,7 @@ the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every 
     python -m bundlefusion_b200.scan scan.sens out.ply [--frames N] [--device cuda:0] [--solve-frames-before-exit 30]
         [--mesh-voxel-size V]       after the loop, fuse its frames along the final trajectory into a V-sized hash and mesh that (bundlefusion_b200.fuse)
         [--poses recorded]          no loop: fuse along the poses stored with the frames (the reference's s_binaryDumpSensorUseTrajectory)
+        [--fit-hash]                size that fused hash from a count of the blocks it will hold (fuse.fit_hash_params), so it drops nothing
 """
 from __future__ import annotations
 
@@ -33,12 +34,13 @@ class _LoopScene:
 
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
                 sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None,
-                mesh_voxel_size: float | None = None) -> dict:
+                mesh_voxel_size: float | None = None, fit_hash: bool = False) -> dict:
     """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
     solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
     global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
     None runs a fixed submapSize + 2 past-end turns.  mesh_voxel_size=V: the loop's frames are then fused along its final trajectory into a
-    fresh hash of voxel size V (FrameLoop.fuse) and that model is meshed instead of the online one; that call's info goes under "fuse"."""
+    fresh hash of voxel size V (FrameLoop.fuse) and that model is meshed instead of the online one; that call's info goes under "fuse".  With
+    fit_hash that hash is sized by FrameLoop.fit_hash_params, whose report goes under "fit"."""
     r = SensorDataReader(sens_path)
     n = len(r) if max_frames is None else min(len(r), max_frames)
     P = fuse.recording_params(r.header, n)
@@ -70,7 +72,11 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
     if finish is not None:
         out["finish"] = finish
     if mesh_voxel_size is not None:
-        scene = CUDASceneRepHashSDF(fuse.fine_hash_params(P, mesh_voxel_size), device)
+        if fit_hash:
+            hp, out["fit"] = loop.fit_hash_params(mesh_voxel_size, n=n)
+        else:
+            hp = fuse.fine_hash_params(P, mesh_voxel_size)
+        scene = CUDASceneRepHashSDF(hp, device)
         out["fuse"] = loop.fuse(scene, n=n)
         if ply_path is not None:
             out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles))
@@ -125,16 +131,26 @@ def main(argv=None) -> int:
                     help="fuse the frames again along the final trajectory into a hash of voxel size V (metres, e.g. 0.004) and mesh that instead of the online model")
     ap.add_argument("--poses", choices=("recorded",), default=None,
                     help="'recorded': no bundling -- fuse along the poses stored with the frames (at --mesh-voxel-size, default the loop's 1 cm) and mesh that")
+    ap.add_argument("--fit-hash", action="store_true",
+                    help="with --mesh-voxel-size or --poses recorded: count the blocks the fusion will allocate and size its hash from the count, so that "
+                         "no insert is dropped (the JSON summary carries the report under 'fit')")
     a = ap.parse_args(argv)
+    if a.fit_hash and a.poses != "recorded" and a.mesh_voxel_size is None:
+        ap.error("--fit-hash sizes a fused hash: use it with --mesh-voxel-size or --poses recorded")
     if a.poses == "recorded":
+        if a.fit_hash and (a.hash_buckets is not None or a.sdf_blocks is not None):
+            ap.error("--fit-hash sizes the fused hash itself: drop --hash-buckets / --sdf-blocks")
         voxel = a.mesh_voxel_size if a.mesh_voxel_size is not None else float(default_params(16, 16).hash.m_virtualVoxelSize)
-        o = fuse.fuse_recording(a.sens, a.ply, voxel, "recorded", a.hash_buckets, a.sdf_blocks, a.device, a.frames)
+        o = fuse.fuse_recording(a.sens, a.ply, voxel, "recorded", a.hash_buckets, a.sdf_blocks, a.device, a.frames, fit_hash=a.fit_hash)
         o["scene"].close()
-        print(json.dumps({"frames": o["frames"], "fuse": {k: o[k] for k in ("fused", "skipped", "batches", "inserts_dropped", "heap_free")},
-                          "triangles": o["triangles"], "mesh_path": o["mesh_path"]}))
+        summary = {"frames": o["frames"], "fuse": {k: o[k] for k in ("fused", "skipped", "batches", "inserts_dropped", "heap_free")},
+                   "triangles": o["triangles"], "mesh_path": o["mesh_path"]}
+        if "fit" in o:
+            summary["fit"] = o["fit"]
+        print(json.dumps(summary))
         return 0
     o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit,
-                    mesh_voxel_size=a.mesh_voxel_size)
+                    mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
     summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path")}
@@ -142,6 +158,8 @@ def main(argv=None) -> int:
         summary["finish"] = o["finish"]                     # its "valid": StopScanningAndExit's verdict on the reconstruction
     if "fuse" in o:
         summary["fuse"] = {k: o["fuse"][k] for k in ("frames_fused", "frames_skipped", "batches", "inserts_dropped", "heap_free")}
+    if "fit" in o:
+        summary["fit"] = o["fit"]
     gt = recorded_poses(a.sens, a.frames)
     if np.isfinite(gt).all(axis=(1, 2)).sum() >= 3:
         summary["ate"] = ate(o["trajectory"], gt[:len(o["trajectory"])])

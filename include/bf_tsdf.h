@@ -257,6 +257,41 @@ int bfTsdfSetBatching(int enable);
 int bfTsdfIntegrateBatch(BFHashDataStruct* hashData, BFHashParams* hashParams, const BFDepthCameraParams* depthCameraParams,
                          const int32_t* frames, const float* poses, int n, const float* const* d_depthFrames, const uint8_t* const* d_colorFrames);
 
+/* Sizing a hash from the blocks a fusion will allocate.
+ *
+ * BFBlockKeySet: a caller-owned device set of SDF-block positions.  d_keys holds `capacity` (a power of two, <= 2^31) 64-bit slots, 0 = empty;
+ * a stored key is bit 63 | (x + 2^20) << 42 | (y + 2^20) << 21 | (z + 2^20).  d_counters[0] = distinct keys stored, [1] = keys refused because
+ * every slot held another key (nothing is written for them: grow the set -- bfTsdfBlockKeyMerge into a larger one -- and count those frames
+ * again), [2] = blocks with a coordinate outside [-2^20, 2^20) that no key can hold.  Zero d_keys and d_counters before the first call; calls
+ * accumulate, so a recording can be counted 16 frames at a time from a ring of device slots.
+ *
+ * bfTsdfCountBlocks adds to the set every block that bfTsdfIntegrateBatch's alloc launches would insert for frames[k] at poses[k] (same
+ * arguments, hashParams the pose-independent parameters): the same walk compiled with another sink, the pose and its inverse formed on the
+ * host as bfTsdfIntegrateBatch forms them, the same frustum test, depth validity and m_maxIntegrationDistance, and the same shard ownership
+ * under m_dummy = {rank, world}.  The hash's sizes are not read.
+ *
+ * bfTsdfBlockKeyLoad writes d_out[0] = keys in the set, d_out[1] = the largest load of any of numBuckets buckets under the hash's own bucket
+ * function, d_out[2] = over = sum over buckets of max(0, load - BF_HASH_BUCKET_SIZE); d_bucketLoad (numBuckets words) receives the loads.
+ *
+ * The guarantee: the blocks live in a hash fused from an empty state by bfTsdfIntegrateBatch / bfFrameLoopFuse over the counted frames and
+ * poses are always a subset of the counted union, garbage collection included (GC only removes blocks).  With numBuckets such that over == 0
+ * and m_numSDFBlocks >= d_counters[0], every insert therefore finds a free slot in its home bucket: no overflow list, no probe, no drop, and
+ * the heap cannot run out.  When over > 0 nothing is claimed beyond what bfTsdfGetLastFrameStats reports after the fusion.
+ *
+ * All three return cudaErrorInvalidValue with nothing enqueued for: n < 1 or n > 16, NULL set / keys / counters / hashParams / camera / frames /
+ * poses / depth array, a negative frame index or NULL depth pointer, a capacity that is 0, not a power of two or above 2^31, numBuckets == 0,
+ * NULL d_bucketLoad / d_out, and merging a set into itself.  Asynchronous on the library stream. */
+typedef struct BFBlockKeySet {
+    uint64_t* d_keys;
+    uint32_t* d_counters;     /* [3] */
+    uint32_t  capacity;
+} BFBlockKeySet;
+int bfTsdfCountBlocks(BFBlockKeySet* set, const BFHashParams* hashParams, const BFDepthCameraParams* depthCameraParams, const int32_t* frames,
+                      const float* poses, int n, const float* const* d_depthFrames);
+int bfTsdfBlockKeyLoad(const BFBlockKeySet* set, uint32_t numBuckets, uint32_t* d_bucketLoad, uint32_t* d_out);
+/* every key of src into dst (growing a set); src's counters are not read */
+int bfTsdfBlockKeyMerge(BFBlockKeySet* dst, const BFBlockKeySet* src);
+
 /* CUDASceneRepHashSDF::garbageCollect (h:110-126) over the last compactified list */
 int bfTsdfGarbageCollect(BFHashDataStruct* hashData, const BFHashParams* hashParams);
 
