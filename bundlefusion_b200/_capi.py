@@ -108,7 +108,7 @@ TSDF_SYMBOLS = [
     "bfSetStream", "bfGetStream", "bfGetLastErrorString", "bfTsdfAuxBytes", "bfTsdfReset", "bfTsdfIntegrateFrame",
     "bfTsdfGarbageCollect", "bfTsdfGetHeapFreeCount", "bfTsdfGetNumOccupiedBlocks", "bfTsdfGetLastFrameStats",
     "bfTsdfReleaseAux", "bfTsdfReintegrateFrame", "bfGetLaunchCount", "bfTsdfSetProfiling", "bfTsdfGetProfile", "bfTsdfGetProfileEx", "bfTsdfSetLanes", "bfTsdfSetArithmetic", "bfTsdfReintegrateBatch", "bfTsdfSetBatching",
-    "bfTsdfIntegrateBatch", "bfTsdfCountBlocks", "bfTsdfBlockKeyLoad", "bfTsdfBlockKeyMerge",
+    "bfTsdfIntegrateBatch", "bfTsdfCountBlocks", "bfTsdfBlockKeyLoad", "bfTsdfBlockKeyMerge", "bfTsdfRehash",
 ]
 
 HOST_SYMBOLS = ["bfMat4Inverse", "bfTsdfRunOps"]
@@ -323,6 +323,7 @@ def lib() -> C.CDLL:
     L.bfTsdfCountBlocks.argtypes = [P(BFBlockKeySet), P(BFHashParams), P(BFDepthCameraParams), vp, vp, C.c_int, vp]
     L.bfTsdfBlockKeyLoad.argtypes = [P(BFBlockKeySet), C.c_uint32, vp, vp]
     L.bfTsdfBlockKeyMerge.argtypes = [P(BFBlockKeySet), P(BFBlockKeySet)]
+    L.bfTsdfRehash.argtypes = [P(BFHashDataStruct), P(BFHashParams), P(BFHashDataStruct), P(BFHashParams), P(C.c_ulonglong)]
     # solver
     L.solveBundlingStub.argtypes = [P(BFSolverInput), P(BFSolverState), P(BFSolverParameters), P(BFSolverStateAnalysis), P(C.c_float), vp]
     L.solveBundlingStub.restype = None

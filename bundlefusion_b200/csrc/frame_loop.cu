@@ -32,6 +32,7 @@
 
 namespace bf {
 int tsdf_batching_usable();          // tsdf.cu: batching on and fast arithmetic selected (bfTsdfRunOps' rule)
+int tsdf_stats_async(const BFHashDataStruct* hd, unsigned* h_out);     // tsdf.cu: heap counter + drop counters into pinned memory, no host wait
 
 extern unsigned long long g_launchCount;
 
@@ -256,6 +257,14 @@ struct Loop {
     bool profile = false; cudaEvent_t stageEv[BF_FRAMELOOP_STAGES + 1] = {}; bool stageHit[BF_FRAMELOOP_STAGES + 1] = {}; double stageMs[BF_FRAMELOOP_STAGES] = {}; unsigned long long profiledSteps = 0;
     // op log (bfFrameLoopSetOpLog): every TSDF op reconstruct() hands to bfTsdfRunOps, with the turn (step or past-end turn, counted from 0) that issued it
     bool opLogOn = false; unsigned turn = 0; std::vector<BFTsdfOp> opLog; std::vector<uint32_t> opLogTurn;
+    // hash growth (bfFrameLoopGetHashGrowth): the table's buffers are stream-ordered allocations the loop owns (not the arena's); h_hashStat
+    // receives {heap counter, heap failures, drops} of the turn statTurn, evHashStat marks its arrival
+    struct Growth {
+        bool on = false, ceilingReached = false, pending = false, sampled = false;
+        unsigned growths = 0, discarded = 0, initBlocks = 0, initBuckets = 0, bucketScale = 1;
+        unsigned* h_stat = nullptr; cudaEvent_t ev = nullptr; unsigned statTurn = 0, statBlocks = 0;
+        unsigned live = 0, sampleTurn = 0, maxInc = 0; unsigned long long dropped = 0; bool dropRose = false;
+    } grow;
 };
 // boundary k = end of stage k - 1 / start of stage k
 static void mark(Loop& L, int k) { if (L.profile && L.stageEv[k]) { cudaEventRecord(L.stageEv[k], stream()); L.stageHit[k] = true; } }
@@ -726,6 +735,109 @@ static int optimize_global(Loop& L) {
     return 0;
 }
 
+// ---- hash growth (bf_frameloop.h, bfFrameLoopGetHashGrowth) --------------------------------------------------------------------------
+// the buffers of a voxel hash of hp's sizes, as stream-ordered allocations on the library stream (bfTsdfReset initialises them); the
+// d_hashDecision arrays and the list counter start zeroed, as the arena's do
+static void hash_free(BFHashDataStruct& hd) {
+    void* p[9] = { hd.d_heap, hd.d_heapCounter, hd.d_hashDecision, hd.d_hashDecisionPrefix, hd.d_hash, hd.d_hashCompactified, hd.d_hashCompactifiedCounter,
+                   hd.d_SDFBlocks, hd.d_hashBucketMutex };
+    for (void* q : p) if (q) cudaFreeAsync(q, stream());
+    memset(&hd, 0, sizeof(hd));
+}
+static int hash_alloc(BFHashDataStruct& hd, const BFHashParams& hp) {
+    memset(&hd, 0, sizeof(hd));
+    const size_t nE = (size_t)hp.m_hashNumBuckets * BF_HASH_BUCKET_SIZE;
+    struct { void** p; size_t bytes; bool zero; } b[9] = {
+        { (void**)&hd.d_heap, sizeof(uint32_t) * (size_t)hp.m_numSDFBlocks, false }, { (void**)&hd.d_heapCounter, sizeof(uint32_t), true },
+        { (void**)&hd.d_hashDecision, sizeof(int32_t) * nE, true }, { (void**)&hd.d_hashDecisionPrefix, sizeof(int32_t) * nE, true },
+        { (void**)&hd.d_hash, sizeof(BFHashEntry) * nE, false }, { (void**)&hd.d_hashCompactified, sizeof(BFHashEntry) * nE, false },
+        { (void**)&hd.d_hashCompactifiedCounter, sizeof(int32_t), true }, { (void**)&hd.d_SDFBlocks, sizeof(BFVoxel) * BF_SDF_BLOCK_VOXELS * (size_t)hp.m_numSDFBlocks, false },
+        { (void**)&hd.d_hashBucketMutex, sizeof(int32_t) * (size_t)hp.m_hashNumBuckets, false } };
+    for (auto& x : b) {
+        cudaError_t e = cudaMallocAsync(x.p, x.bytes, stream());
+        if (e == cudaSuccess && x.zero) e = cudaMemsetAsync(*x.p, 0, x.bytes, stream());
+        if (e != cudaSuccess) { set_last_error("frame loop: hash growth allocation", e); hash_free(hd); return (int)e; }
+    }
+    hd.m_bIsOnGPU = 1;
+    return 0;
+}
+
+// the growth-size rule (bfFrameLoopHashGrowthSize): heap = min(ceiling, max(2 x old, live + 2 x reserve)); buckets at the initial ratio, odd,
+// within the 32-bit entry-index limit
+static unsigned grown_blocks(unsigned blocks, unsigned live, unsigned long long reserve, unsigned ceiling) {
+    return (unsigned)std::min<unsigned long long>(std::max<unsigned long long>(2ull * blocks, live + 2ull * reserve), ceiling);
+}
+static unsigned grown_buckets(unsigned initBlocks, unsigned initBuckets, unsigned blocks) {
+    const unsigned long long nb = (unsigned long long)initBuckets * blocks / std::max(initBlocks, 1u);
+    return (unsigned)std::min<unsigned long long>(nb | 1ull, 0xFFFFFFFFull / BF_HASH_BUCKET_SIZE);
+}
+
+static int join_tsdf(Loop& L);
+// Move the model into a table of `blocks` voxel blocks (buckets at the initial bucket-to-block ratio), before turn `turn`'s op list runs.
+static int grow_hash(Loop& L, unsigned blocks, unsigned turn) {
+    Loop::Growth& G = L.grow;
+    FL_OK(join_tsdf(L));                                        // the old table's last work, queued on the reconstruction stream, comes first
+    const unsigned long long cap = 0xFFFFFFFFull / BF_HASH_BUCKET_SIZE;
+    for (int attempt = 0; attempt < 3; ++attempt) {
+        BFHashParams hp = L.hp;
+        const unsigned initBuckets = (unsigned)std::min<unsigned long long>((unsigned long long)G.initBuckets * G.bucketScale, cap);
+        hp.m_numSDFBlocks = blocks; hp.m_hashNumBuckets = std::max(grown_buckets(G.initBlocks, initBuckets, blocks), L.hp.m_hashNumBuckets);
+        BFHashDataStruct hd;
+        FL_OK(hash_alloc(hd, hp));
+        unsigned long long moved[2] = { 0, 0 };
+        int rc = bfTsdfReset(&hd, &hp);
+        if (!rc) rc = bfTsdfRehash(&L.hd, &L.hp, &hd, &hp, moved);
+        L.counters[6] += BF_FRAMELOOP_GROWTH_SYNCS;
+        if (rc) { bfTsdfReleaseAux(&hd); hash_free(hd); return rc; }
+        if (moved[1] == 0) {
+            bfTsdfReleaseAux(&L.hd);
+            hash_free(L.hd);
+            L.hd = hd; L.hp = hp;
+            ++G.growths;
+            // bfTsdfRehash synchronised: an exact sample of the state after the previous turn; a read-back still in flight is older
+            G.pending = false; G.live = (unsigned)moved[0]; G.sampleTurn = turn - 1; G.dropRose = false;
+            return 0;
+        }
+        // the new table's probe windows could not take every live block: discard it and keep the old one, which the rehash only read, and
+        // try again with twice the buckets per block (kept for later growths)
+        bfTsdfReleaseAux(&hd); hash_free(hd);
+        ++G.discarded;
+        if (hp.m_hashNumBuckets >= cap) break;
+        G.bucketScale *= 2;
+    }
+    G.dropRose = false;                                         // no table took the model: the loop goes on with the old one
+    return 0;
+}
+
+// At the start of turn `turn`'s reconstruction: take the last read-back if it has arrived (never waiting for it), then grow if the free
+// blocks it saw are below the reserve or the dropped count rose.
+static int maybe_grow(Loop& L, unsigned turn) {
+    Loop::Growth& G = L.grow;
+    if (G.pending) {
+        const cudaError_t q = cudaEventQuery(G.ev);
+        if (q == cudaErrorNotReady) cudaGetLastError();        // not an error: the read-back is still in flight
+        else {
+            BF_CHECK(q);
+            G.pending = false;
+            const unsigned c = G.h_stat[0];
+            const unsigned freeBlocks = c >= 0x80000000u ? 0u : std::min(c + 1u, G.statBlocks);
+            const unsigned live = G.statBlocks - freeBlocks;
+            const unsigned long long dropped = (unsigned long long)G.h_stat[1] + G.h_stat[2];
+            const unsigned before = G.sampled ? G.live : 0u;
+            if (live > before) G.maxInc = std::max(G.maxInc, live - before);
+            if (dropped > G.dropped) G.dropRose = true;
+            G.live = live; G.dropped = dropped; G.sampleTurn = G.statTurn; G.sampled = true;
+        }
+    }
+    if (!G.sampled) return 0;
+    const unsigned blocks = L.hp.m_numSDFBlocks;
+    const unsigned long long reserve = 2ull * G.maxInc * std::max(1u, turn - G.sampleTurn);
+    if (!((unsigned long long)(blocks - std::min(G.live, blocks)) < reserve || G.dropRose)) return 0;
+    const unsigned want = grown_blocks(blocks, G.live, reserve, L.P.hashMaxSDFBlocks);
+    if (want <= blocks) { G.ceilingReached = true; G.dropRose = false; return 0; }
+    return grow_hash(L, want, turn);
+}
+
 // reintegrate() (FL/DepthSensing/DepthSensing.cpp:854-902) + the integration of the current frame (:1033-1061): one op list, one bfTsdfRunOps
 static int reconstruct(Loop& L, bool gotFrame, unsigned curFrame) {
     const BFFrameLoopParams& P = L.P;
@@ -763,11 +875,17 @@ static int reconstruct(Loop& L, bool gotFrame, unsigned curFrame) {
     const unsigned turn = L.turn++;
     if (P.reconstructionEnabled) {
         if (L.opLogOn) { L.opLog.insert(L.opLog.end(), ops.begin(), ops.end()); L.opLogTurn.insert(L.opLogTurn.end(), ops.size(), turn); }
+        if (L.grow.on) FL_OK(maybe_grow(L, turn));
         // inputs of this call that live on the main stream: the frame store (ingest of this frame) -- the poses and the op list are host data
         const bool side = L.overlap && !L.profile && L.tsdfStream;
         cudaStream_t mainStream = stream();
         if (side) { BF_CHECK(cudaEventRecord(L.evMain, mainStream)); BF_CHECK(cudaStreamWaitEvent(L.tsdfStream, L.evMain, 0)); bfSetStream(L.tsdfStream); }
-        const int rc = bfTsdfRunOps(&L.hd, &L.hp, &L.cam, ops.data(), (int)ops.size(), L.depthPtrs.data(), L.colorPtrs.data());
+        int rc = bfTsdfRunOps(&L.hd, &L.hp, &L.cam, ops.data(), (int)ops.size(), L.depthPtrs.data(), L.colorPtrs.data());
+        if (!rc && L.grow.on && !L.grow.pending) {              // read back this turn's heap and drop counters behind its work
+            rc = tsdf_stats_async(&L.hd, L.grow.h_stat);
+            if (!rc) rc = (int)cudaEventRecord(L.grow.ev, stream());
+            L.grow.pending = rc == 0; L.grow.statTurn = turn; L.grow.statBlocks = L.hp.m_numSDFBlocks;
+        }
         if (side) { cudaEventRecord(L.evTsdf, L.tsdfStream); L.tsdfPending = true; bfSetStream(mainStream); }
         if (rc) return rc;
     }
@@ -794,6 +912,15 @@ static int bundler_init(Loop& L, Bundler& b, bool isLocal, unsigned maxImages) {
     fl_set_identity_kernel<<<((maxImages + 1) * 16 + 255) / 256, 256, 0, stream()>>>(b.d_trajectory, maxImages + 1);
     BF_CHECK(cudaGetLastError());
     return 0;
+}
+
+// a growing loop's table, read-back slot and event (bfFrameLoopDestroy, or a failed bfFrameLoopCreate)
+static void release_grown_hash(Loop& L) {
+    bfTsdfReleaseAux(&L.hd);
+    hash_free(L.hd);
+    cudaStreamSynchronize(stream());
+    if (L.grow.h_stat) cudaFreeHost(L.grow.h_stat);
+    if (L.grow.ev) cudaEventDestroy(L.grow.ev);
 }
 
 static void fill_status_tail(Loop& L) {
@@ -892,14 +1019,23 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
         L.hp = P.hash; L.hp.m_hashBucketSize = BF_HASH_BUCKET_SIZE; L.hp.m_SDFBlockSize = BF_SDF_BLOCK_SIZE;
         const size_t nEntries = (size_t)L.hp.m_hashNumBuckets * BF_HASH_BUCKET_SIZE;
         memset(&L.hd, 0, sizeof(L.hd));
-        L.hd.d_heap = L.A.get<uint32_t>(L.hp.m_numSDFBlocks, false); L.hd.d_heapCounter = L.A.get<uint32_t>(1);
-        L.hd.d_hashDecision = L.A.get<int32_t>(nEntries); L.hd.d_hashDecisionPrefix = L.A.get<int32_t>(nEntries);
-        L.hd.d_hash = L.A.get<BFHashEntry>(nEntries, false); L.hd.d_hashCompactified = L.A.get<BFHashEntry>(nEntries, false);
-        L.hd.d_hashCompactifiedCounter = L.A.get<int32_t>(1);
-        L.hd.d_SDFBlocks = L.A.get<BFVoxel>((size_t)L.hp.m_numSDFBlocks * BF_SDF_BLOCK_VOXELS, false);
-        L.hd.d_hashBucketMutex = L.A.get<int32_t>(L.hp.m_hashNumBuckets, false);
-        L.hd.m_bIsOnGPU = 1;
-        if (L.A.err) { rc = L.A.err; break; }
+        L.grow.on = P.hashMaxSDFBlocks > L.hp.m_numSDFBlocks && L.hp.m_numSDFBlocks > 0;
+        if (L.grow.on) {                 // a table the loop may replace: its own stream-ordered buffers, a pinned read-back slot and its event
+            L.grow.initBlocks = L.hp.m_numSDFBlocks; L.grow.initBuckets = L.hp.m_hashNumBuckets;
+            if ((rc = hash_alloc(L.hd, L.hp))) break;
+            cudaError_t e = cudaMallocHost(&L.grow.h_stat, 4 * sizeof(unsigned));
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&L.grow.ev, cudaEventDisableTiming);
+            if (e != cudaSuccess) { rc = (int)e; break; }
+        } else {
+            L.hd.d_heap = L.A.get<uint32_t>(L.hp.m_numSDFBlocks, false); L.hd.d_heapCounter = L.A.get<uint32_t>(1);
+            L.hd.d_hashDecision = L.A.get<int32_t>(nEntries); L.hd.d_hashDecisionPrefix = L.A.get<int32_t>(nEntries);
+            L.hd.d_hash = L.A.get<BFHashEntry>(nEntries, false); L.hd.d_hashCompactified = L.A.get<BFHashEntry>(nEntries, false);
+            L.hd.d_hashCompactifiedCounter = L.A.get<int32_t>(1);
+            L.hd.d_SDFBlocks = L.A.get<BFVoxel>((size_t)L.hp.m_numSDFBlocks * BF_SDF_BLOCK_VOXELS, false);
+            L.hd.d_hashBucketMutex = L.A.get<int32_t>(L.hp.m_hashNumBuckets, false);
+            L.hd.m_bIsOnGPU = 1;
+            if (L.A.err) { rc = L.A.err; break; }
+        }
         memset(&L.cam, 0, sizeof(L.cam));
         // integration camera: depth intrinsics scaled to the integration resolution (CUDAImageManager: m_depthIntrinsics adapted, cpp:60-70)
         L.cam.fx = P.depthIntrinsics[0] * (float)P.integrationWidth / (float)P.depthWidth; L.cam.fy = P.depthIntrinsics[5] * (float)P.integrationHeight / (float)P.depthHeight;
@@ -920,7 +1056,13 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
         e = cudaStreamSynchronize(stream());
         if (e != cudaSuccess) { rc = (int)e; break; }
     } while (0);
-    if (rc) { if (L.tm) bfTrajectoryDestroy(L.tm); if (L.h_pin) cudaFreeHost(L.h_pin); if (L.h_complete) cudaFreeHost(L.h_complete); delete Lp; return rc; }
+    if (rc) {
+        if (L.tm) bfTrajectoryDestroy(L.tm);
+        if (L.h_pin) cudaFreeHost(L.h_pin);
+        if (L.h_complete) cudaFreeHost(L.h_complete);
+        if (L.grow.on) release_grown_hash(L);
+        delete Lp; return rc;
+    }
     *out = reinterpret_cast<BFFrameLoop*>(Lp);
     return 0;
 }
@@ -932,6 +1074,7 @@ BF_API void bfFrameLoopDestroy(BFFrameLoop* loop) {
     if (L->featStream) cudaStreamSynchronize(L->featStream);
     cudaStreamSynchronize(stream());
     bfTsdfReleaseAux(&L->hd);
+    if (L->grow.on) release_grown_hash(*L);
     if (L->tsdfStream) cudaStreamDestroy(L->tsdfStream);
     if (L->featStream) cudaStreamDestroy(L->featStream);
     if (L->evStepStart) cudaEventDestroy(L->evStepStart);
@@ -1215,6 +1358,24 @@ BF_API int bfFrameLoopSetOverlap(BFFrameLoop* loop, int enable) {
     return prev;
 }
 BF_API const BFHashParams* bfFrameLoopGetHashParams(const BFFrameLoop* loop) { return loop ? &reinterpret_cast<const Loop*>(loop)->hp : nullptr; }
+BF_API void bfFrameLoopHashGrowthSize(uint32_t blocks, uint32_t live, unsigned long long reserve, uint32_t ceiling, uint32_t initBlocks, uint32_t initBuckets,
+                                      uint32_t* newBlocks, uint32_t* newBuckets) {
+    const unsigned b = grown_blocks(blocks, live, reserve, ceiling);
+    if (newBlocks) *newBlocks = b;
+    if (newBuckets) *newBuckets = grown_buckets(initBlocks, initBuckets, b);
+}
+BF_API int bfFrameLoopGetHashGrowth(BFFrameLoop* loop, BFFrameLoopHashGrowth* out) {
+    if (!loop || !out) return (int)cudaErrorInvalidValue;
+    Loop& L = *reinterpret_cast<Loop*>(loop);
+    FL_OK(join_tsdf(L));
+    unsigned long long st[4] = { 0, 0, 0, 0 };
+    FL_OK(bfTsdfGetLastFrameStats(&L.hd, st));          // out[3]: drops since the reset, carried across every rehash
+    memset(out, 0, sizeof(*out));
+    out->growths = L.grow.growths; out->discarded = L.grow.discarded; out->sdfBlocks = L.hp.m_numSDFBlocks; out->buckets = L.hp.m_hashNumBuckets;
+    out->maxSDFBlocks = L.grow.on ? L.P.hashMaxSDFBlocks : L.hp.m_numSDFBlocks;
+    out->insertsDropped = st[3]; out->ceilingReached = L.grow.ceilingReached ? 1 : 0;
+    return 0;
+}
 BF_API int bfFrameLoopSetProfiling(BFFrameLoop* loop, int enable) {
     if (!loop) return (int)cudaErrorInvalidValue;
     Loop& L = *reinterpret_cast<Loop*>(loop);

@@ -27,6 +27,7 @@
 #include "bf_common.cuh"
 #include "tsdf_shared.cuh"
 #include "tsdf_keys.cuh"
+#include "tsdf_hash.cuh"
 #include "mat4.cuh"
 
 namespace bf {
@@ -158,150 +159,6 @@ __device__ __forceinline__ bool block_in_frustum_m(float vs, const BFFloat4x4& M
     float iz = proj_z(cp, pc.z);
     ix *= 0.95f; iy *= 0.95f; iz *= 0.95f;
     return !(ix < -1.0f || ix > 1.0f || iy < -1.0f || iy > 1.0f || iz < 0.0f || iz > 1.0f);
-}
-
-// ------------------------------------------------------------------------------------------
-// hash table primitives.  Entry = 5 ints (20 B).  Loads on the lock-free fast path may come
-// from L1 (possibly stale => at worst a spurious miss that is re-checked under the lock);
-// loads under a bucket lock use ld.global.cg (L2), stores are followed by __threadfence().
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool entry_matches(const BFHashEntry* e, I3 p) {
-    return e->pos[0] == p.x && e->pos[1] == p.y && e->pos[2] == p.z && e->ptr != BF_FREE_ENTRY;
-}
-__device__ __forceinline__ BFHashEntry load_entry_cg(const BFHashEntry* e) {
-    BFHashEntry r;
-    const int* s = reinterpret_cast<const int*>(e);
-    r.pos[0] = __ldcg(s + 0); r.pos[1] = __ldcg(s + 1); r.pos[2] = __ldcg(s + 2); r.ptr = __ldcg(s + 3);
-    r.offset = (unsigned)__ldcg(s + 4);
-    return r;
-}
-__device__ __forceinline__ bool entry_matches_v(const BFHashEntry& e, I3 p) {
-    return e.pos[0] == p.x && e.pos[1] == p.y && e.pos[2] == p.z && e.ptr != BF_FREE_ENTRY;
-}
-
-// VoxelUtilHashSDF.h:440-485 ; returns entry index or -1.  kCoherent: read through L2.
-template <bool kCoherent>
-__device__ int find_entry(const BFHashEntry* __restrict__ hash, const BFHashParams& hp, I3 p, unsigned h) {
-    const unsigned hpz = h * BF_HASH_BUCKET_SIZE;
-    const unsigned total = BF_HASH_BUCKET_SIZE * hp.m_hashNumBuckets;
-#pragma unroll
-    for (unsigned j = 0; j < BF_HASH_BUCKET_SIZE; ++j) {
-        if (kCoherent) { if (entry_matches_v(load_entry_cg(&hash[hpz + j]), p)) return (int)(hpz + j); }
-        else           { if (entry_matches(&hash[hpz + j], p)) return (int)(hpz + j); }
-    }
-    const unsigned last = hpz + BF_HASH_BUCKET_SIZE - 1;
-    unsigned i = last;
-    for (unsigned it = 0; it < hp.m_hashMaxCollisionLinkedListSize; ++it) {
-        BFHashEntry c = kCoherent ? load_entry_cg(&hash[i]) : hash[i];
-        if (entry_matches_v(c, p)) return (int)i;
-        if (c.offset == 0) break;
-        i = (last + c.offset) % total;
-    }
-    return -1;
-}
-
-__device__ __forceinline__ bool try_lock(int* mutex) { return atomicCAS(mutex, BF_FREE_ENTRY, BF_LOCK_ENTRY) == BF_FREE_ENTRY; }
-__device__ __forceinline__ void unlock(int* mutex) { __threadfence(); atomicExch(mutex, BF_FREE_ENTRY); }
-
-// VoxelUtilHashSDF.h:535-540 consumeHeap, plus an exhaustion guard (the reference has none)
-__device__ __forceinline__ bool heap_pop(unsigned* heap, unsigned* heapCounter, unsigned* slot) {
-    unsigned addr = atomicSub(heapCounter, 1u);
-    if (addr == 0xFFFFFFFFu || addr >= 0x80000000u) { atomicAdd(heapCounter, 1u); return false; }
-    *slot = __ldcg(&heap[addr]);
-    return true;
-}
-
-__device__ __forceinline__ void write_entry(BFHashEntry* e, I3 p, unsigned offset, int ptr) {
-    int* d = reinterpret_cast<int*>(e);
-    __stcg(d + 0, p.x); __stcg(d + 1, p.y); __stcg(d + 2, p.z); __stcg(d + 4, (int)offset);
-    __threadfence();
-    __stcg(d + 3, ptr);       // ptr last: a reader that sees a valid ptr sees a valid pos
-}
-
-// Insert `pos` (VoxelUtilHashSDF.h:549-655 semantics: bucket slot first, else splice into the
-// bucket's overflow list).  Unlike the reference (try-lock, give up, host retries) this spins
-// until the block is present, so one launch reaches the reference's fixed point.
-// slotEpoch / tag (optional): batch re-integration -- a block inserted by THIS launch is tagged with (batch id << 8 | op index), so that the
-// multi-op stencil can tell which operations of the batch saw the block exist (tsdf_reintegrate_batch)
-struct AllocEpoch { unsigned* slotEpoch; unsigned tag; };
-__device__ void alloc_block(const BFHashDataStruct& hd, const BFHashParams& hp, int4* slotInfo, unsigned* ctrs, I3 pos, AllocEpoch ep = AllocEpoch{nullptr, 0u}) {
-    const unsigned h = hash_pos(hp.m_hashNumBuckets, pos);
-    if (find_entry<false>(hd.d_hash, hp, pos, h) >= 0) return;      // fast path, no lock
-
-    const unsigned hpz = h * BF_HASH_BUCKET_SIZE;
-    const unsigned last = hpz + BF_HASH_BUCKET_SIZE - 1;
-    const unsigned total = BF_HASH_BUCKET_SIZE * hp.m_hashNumBuckets;
-    const unsigned maxLoop = hp.m_hashMaxCollisionLinkedListSize;
-    int* mutexH = &hd.d_hashBucketMutex[h];
-
-    bool done = false;
-    unsigned backoff = 32;
-    while (!done) {
-        if (try_lock(mutexH)) {
-            __threadfence();
-            if (find_entry<true>(hd.d_hash, hp, pos, h) >= 0) { unlock(mutexH); return; }
-            // first free slot of the home bucket
-            int firstEmpty = -1;
-#pragma unroll
-            for (unsigned j = 0; j < BF_HASH_BUCKET_SIZE; ++j) {
-                int p = __ldcg(&hd.d_hash[hpz + j].ptr);
-                if (firstEmpty == -1 && p == BF_FREE_ENTRY) firstEmpty = (int)(hpz + j);
-            }
-            if (firstEmpty != -1) {
-                unsigned slot;
-                if (heap_pop(hd.d_heap, hd.d_heapCounter, &slot)) {
-                    slotInfo[slot] = make_int4(pos.x, pos.y, pos.z, firstEmpty);
-                    if (ep.slotEpoch) ep.slotEpoch[slot] = ep.tag;
-                    atomicMax(&ctrs[CTR_HIGH_WATER], slot + 1u);
-                    write_entry(&hd.d_hash[firstEmpty], pos, BF_NO_OFFSET, (int)(slot * BF_SDF_BLOCK_VOXELS));
-                } else {
-                    atomicAdd(&ctrs[CTR_HEAP_FAIL], 1u);
-                }
-                unlock(mutexH);
-                return;
-            }
-            // overflow: probe forward for a free non-bucket-last slot (:614-654)
-            unsigned offset = 0, it = 0;
-            bool retry = false;
-            while (it < maxLoop) {
-                offset++;
-                const unsigned i = (last + offset) % total;
-                if ((offset % BF_HASH_BUCKET_SIZE) == 0) continue;
-                if (__ldcg(&hd.d_hash[i].ptr) == BF_FREE_ENTRY) {
-                    const unsigned h2 = i / BF_HASH_BUCKET_SIZE;
-                    int* mutex2 = &hd.d_hashBucketMutex[h2];
-                    const bool same = (h2 == h);
-                    if (!same && !try_lock(mutex2)) { retry = true; break; }   // avoid lock-order deadlock
-                    __threadfence();
-                    if (__ldcg(&hd.d_hash[i].ptr) == BF_FREE_ENTRY) {
-                        unsigned slot;
-                        if (heap_pop(hd.d_heap, hd.d_heapCounter, &slot)) {
-                            const unsigned lastOffset = (unsigned)__ldcg(reinterpret_cast<const int*>(&hd.d_hash[last]) + 4);
-                            slotInfo[slot] = make_int4(pos.x, pos.y, pos.z, (int)i);
-                            if (ep.slotEpoch) ep.slotEpoch[slot] = ep.tag;
-                            atomicMax(&ctrs[CTR_HIGH_WATER], slot + 1u);
-                            write_entry(&hd.d_hash[i], pos, lastOffset, (int)(slot * BF_SDF_BLOCK_VOXELS));
-                            __threadfence();
-                            __stcg(reinterpret_cast<int*>(&hd.d_hash[last]) + 4, (int)offset);   // publish: head -> new
-                        } else {
-                            atomicAdd(&ctrs[CTR_HEAP_FAIL], 1u);
-                        }
-                        if (!same) unlock(mutex2);
-                        unlock(mutexH);
-                        return;
-                    }
-                    if (!same) unlock(mutex2);
-                    // slot was taken meanwhile: keep probing (does not count as an iteration)
-                    continue;
-                }
-                it++;
-            }
-            unlock(mutexH);
-            if (!retry) { atomicAdd(&ctrs[CTR_DROPPED], 1u); return; }   // no room within the probe window: dropped (as the reference)
-        }
-        __nanosleep(backoff + ((threadIdx.x * 7u) & 63u));     // jitter: break lock-step livelock inside a warp
-        if (backoff < 1024) backoff <<= 1;
-    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1053,63 +910,6 @@ gc_identify_kernel(BFHashDataStruct hd, unsigned count) {
     }
 }
 
-// deleteHashEntryElement (VoxelUtilHashSDF.h:739-826) under the home bucket's spin lock.
-__device__ bool delete_entry(const BFHashDataStruct& hd, const BFHashParams& hp, int4* slotInfo, I3 p) {
-    const unsigned h = hash_pos(hp.m_hashNumBuckets, p);
-    const unsigned hpz = h * BF_HASH_BUCKET_SIZE;
-    const unsigned last = hpz + BF_HASH_BUCKET_SIZE - 1;
-    const unsigned total = BF_HASH_BUCKET_SIZE * hp.m_hashNumBuckets;
-    int* mutexH = &hd.d_hashBucketMutex[h];
-    unsigned backoff = 32;
-    while (!try_lock(mutexH)) { __nanosleep(backoff); if (backoff < 1024) backoff <<= 1; }
-    __threadfence();
-    bool ok = false;
-    BFHashEntry freeE; freeE.pos[0] = freeE.pos[1] = freeE.pos[2] = 0; freeE.ptr = BF_FREE_ENTRY; freeE.offset = 0;
-    for (unsigned j = 0; j < BF_HASH_BUCKET_SIZE && !ok; ++j) {
-        const unsigned i = hpz + j;
-        const BFHashEntry c = load_entry_cg(&hd.d_hash[i]);
-        if (entry_matches_v(c, p)) {
-            const unsigned slot = (unsigned)c.ptr / BF_SDF_BLOCK_VOXELS;
-            const unsigned addr = atomicAdd(hd.d_heapCounter, 1u);            // appendHeap :541-546
-            hd.d_heap[addr + 1] = slot;
-            slotInfo[slot] = make_int4(0, 0, 0, -1);
-            if (c.offset != 0) {
-                const unsigned next = (i + c.offset) % total;
-                const BFHashEntry n = load_entry_cg(&hd.d_hash[next]);
-                hd.d_hash[i] = n;
-                if (n.ptr >= 0) slotInfo[(unsigned)n.ptr / BF_SDF_BLOCK_VOXELS].w = (int)i;   // the moved entry changed index
-                hd.d_hash[next] = freeE;
-            } else {
-                hd.d_hash[i] = freeE;
-            }
-            ok = true;
-        }
-    }
-    if (!ok) {
-        BFHashEntry c = load_entry_cg(&hd.d_hash[last]);
-        unsigned prev = last;
-        unsigned i = (last + c.offset) % total;
-        for (unsigned it = 0; it < hp.m_hashMaxCollisionLinkedListSize; ++it) {
-            c = load_entry_cg(&hd.d_hash[i]);
-            if (entry_matches_v(c, p)) {
-                const unsigned slot = (unsigned)c.ptr / BF_SDF_BLOCK_VOXELS;
-                const unsigned addr = atomicAdd(hd.d_heapCounter, 1u);
-                hd.d_heap[addr + 1] = slot;
-                slotInfo[slot] = make_int4(0, 0, 0, -1);
-                hd.d_hash[i] = freeE;
-                hd.d_hash[prev].offset = c.offset;
-                ok = true;
-                break;
-            }
-            if (c.offset == 0) break;
-            prev = i;
-            i = (last + c.offset) % total;
-        }
-    }
-    unlock(mutexH);
-    return ok;
-}
-
 // free (.cu:648-668) given d_hashDecision
 __global__ void __launch_bounds__(128)
 gc_free_kernel(BFHashDataStruct hd, const __grid_constant__ BFHashParams hp, unsigned count, int4* slotInfo, unsigned* ctrs) {
@@ -1561,7 +1361,20 @@ BF_API int bfTsdfIntegrateBatch(BFHashDataStruct* hd, BFHashParams* hp, const BF
     for (int k = 0; k < n; ++k) { oldPoses[k] = nullptr; newPoses[k] = poses + 16 * (size_t)k; }
     return run_batch(hd, hp, cp, n, frames, oldPoses, newPoses, d_depthFrames, d_colorFrames);
 }
-namespace bf { int tsdf_batching_usable() { return (batching_on() && arith_fast()) ? 1 : 0; } }
+namespace bf {
+int tsdf_batching_usable() { return (batching_on() && arith_fast()) ? 1 : 0; }
+// the frame loop's hash-growth read-back: h_out[0] = heap counter, h_out[1..2] = heap-failure and dropped-insert counters, copied on the
+// library stream into the caller's pinned memory (no host wait)
+int tsdf_stats_async(const BFHashDataStruct* hd, unsigned* h_out) {
+    TsdfAux* aux;
+    int rc = get_aux(hd, nullptr, &aux, false);
+    if (rc) return rc;
+    static_assert(CTR_DROPPED == CTR_HEAP_FAIL + 1, "adjacent drop counters");
+    BF_CHECK(cudaMemcpyAsync(h_out, hd->d_heapCounter, sizeof(unsigned), cudaMemcpyDeviceToHost, g_stream));
+    BF_CHECK(cudaMemcpyAsync(h_out + 1, aux->ctrs + CTR_HEAP_FAIL, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, g_stream));
+    return 0;
+}
+}
 
 static bool key_set_ok(const BFBlockKeySet* set) {
     return set && set->d_keys && set->d_counters && set->capacity != 0 && (set->capacity & (set->capacity - 1)) == 0 && set->capacity <= (1u << 31);
@@ -1618,6 +1431,77 @@ BF_API int bfTsdfGarbageCollect(BFHashDataStruct* hd, const BFHashParams* hp) {
     if (aux->liveValid) gc_live_kernel<<<grid_for((hp->m_numSDFBlocks + 255) / 256, 2), 256, 0, g_stream>>>(*hd, *hp, live_count_ptr(aux), aux->slotInfo, aux->ctrs, aux->live, aux->lastListDual ? aux->listFlags : nullptr);
     else                gc_fused_kernel<<<grid_for(hp->m_numSDFBlocks, 16), 128, 0, g_stream>>>(*hd, *hp, live_count_ptr(aux), aux->slotInfo, aux->ctrs);
     BF_CHECK(cudaGetLastError());
+    return 0;
+}
+
+// bfTsdfRehash: every argument check is on the host and comes before the first CUDA call; each refusal names its reason
+// (bfGetLastErrorString)
+static const char* geometry_mismatch(const BFHashParams* a, const BFHashParams* b) {
+    if (a->m_virtualVoxelSize != b->m_virtualVoxelSize) return "voxel size differs";
+    if (a->m_truncation != b->m_truncation) return "truncation differs";
+    if (a->m_truncScale != b->m_truncScale) return "truncation scale differs";
+    if (a->m_maxIntegrationDistance != b->m_maxIntegrationDistance) return "max integration distance differs";
+    if (a->m_SDFBlockSize != b->m_SDFBlockSize) return "block size differs";
+    if (a->m_hashBucketSize != b->m_hashBucketSize) return "bucket size differs";
+    if (a->m_hashMaxCollisionLinkedListSize != b->m_hashMaxCollisionLinkedListSize) return "linked-list limit differs";
+    if (a->m_dummy[0] != b->m_dummy[0] || a->m_dummy[1] != b->m_dummy[1]) return "shard setting (m_dummy) differs";
+    return nullptr;
+}
+static bool hash_buffers_ok(const BFHashDataStruct* h, const void* (&p)[9]) {
+    const void* q[9] = { h->d_heap, h->d_heapCounter, h->d_hashDecision, h->d_hashDecisionPrefix, h->d_hash, h->d_hashCompactified,
+                         h->d_hashCompactifiedCounter, h->d_SDFBlocks, h->d_hashBucketMutex };
+    for (int i = 0; i < 9; ++i) p[i] = q[i];
+    return h->d_heap && h->d_heapCounter && h->d_hash && h->d_hashCompactified && h->d_hashCompactifiedCounter && h->d_SDFBlocks && h->d_hashBucketMutex;
+}
+static int rehash_refuse(const char* why) {
+    t_lastError = std::string("bfTsdfRehash: ") + why;
+    return (int)cudaErrorInvalidValue;
+}
+
+BF_API int bfTsdfRehash(const BFHashDataStruct* src, const BFHashParams* sp, BFHashDataStruct* dst, const BFHashParams* dp, unsigned long long out[2]) {
+    if (!src || !sp || !dst || !dp || !out) return rehash_refuse("NULL argument");
+    if (src == dst) return rehash_refuse("src == dst");
+    const void* ps[9]; const void* pd[9];
+    if (!hash_buffers_ok(src, ps) || !hash_buffers_ok(dst, pd)) return rehash_refuse("NULL buffer");
+    for (int i = 0; i < 9; ++i)
+        for (int j = 0; j < 9; ++j)
+            if (ps[i] && ps[i] == pd[j]) return rehash_refuse("src and dst share a buffer");
+    if (const char* why = geometry_mismatch(sp, dp)) return rehash_refuse(why);
+    if (dp->m_numSDFBlocks == 0) return rehash_refuse("dst heap size 0");
+    if (dp->m_hashNumBuckets == 0 || dp->m_hashNumBuckets > 0xFFFFFFFFu / BF_HASH_BUCKET_SIZE) return rehash_refuse("dst bucket count 0 or beyond 32-bit entry indices");
+    TsdfAux* sa; TsdfAux* da;
+    if (get_aux(src, sp, &sa, false) != 0) return rehash_refuse("src is not a hash this library maintains (bfTsdfReset)");
+    if (get_aux(dst, dp, &da, false) != 0) return rehash_refuse("dst is not a hash this library maintains (bfTsdfReset)");
+    int rc = join_lanes(sa); if (rc) return rc;
+    // src's live block count and last list length: dst must hold both
+    unsigned h[2] = { 0, 0 };
+    BF_CHECK(cudaMemcpyAsync(&h[0], src->d_heapCounter, sizeof(unsigned), cudaMemcpyDeviceToHost, g_stream));
+    BF_CHECK(cudaMemcpyAsync(&h[1], live_count_ptr(sa), sizeof(unsigned), cudaMemcpyDeviceToHost, g_stream));
+    BF_CHECK(cudaStreamSynchronize(g_stream));
+    const unsigned srcFree = (h[0] >= 0x80000000u || h[0] >= sp->m_numSDFBlocks) ? (h[0] >= 0x80000000u ? 0u : sp->m_numSDFBlocks) : h[0] + 1u;
+    const unsigned live = sp->m_numSDFBlocks - srcFree;
+    if (dp->m_numSDFBlocks < live || h[1] > dp->m_numSDFBlocks || h[1] > dp->m_hashNumBuckets * BF_HASH_BUCKET_SIZE) {
+        return rehash_refuse("dst heap smaller than src's live blocks or its last list");
+    }
+    unsigned* tmp = nullptr;                     // [2] moved / refused, then the slot map
+    BF_CHECK(cudaMallocAsync(&tmp, sizeof(unsigned) * ((size_t)sa->numSlots + 2), g_stream));
+    unsigned* const slotMap = tmp + 2;
+    BF_CHECK(cudaMemsetAsync(tmp, 0, 2 * sizeof(unsigned), g_stream));
+    BF_CHECK(cudaMemsetAsync(slotMap, 0xff, sizeof(unsigned) * (size_t)sa->numSlots, g_stream));
+    ++g_launchCount;
+    rehash_kernel<<<grid_for((sa->numSlots + BF_REHASH_CHUNK - 1) / BF_REHASH_CHUNK, 8), BF_REHASH_CHUNK, 0, g_stream>>>(
+        *src, *dst, *dp, sa->slotInfo, sa->ctrs, sa->live, da->slotInfo, da->ctrs, da->live, slotMap, tmp);
+    BF_CHECK(cudaGetLastError());
+    ++g_launchCount;
+    rehash_list_kernel<<<grid_for((sa->numSlots + 255) / 256, 4), 256, 0, g_stream>>>(*src, *dst, sa->ctrs, da->ctrs, set_of(sa->parity), da->slotInfo, slotMap,
+                                                                                      sa->listFlags, da->listFlags);
+    BF_CHECK(cudaGetLastError());
+    unsigned o[2] = { 0, 0 };
+    BF_CHECK(cudaMemcpyAsync(o, tmp, sizeof(o), cudaMemcpyDeviceToHost, g_stream));
+    BF_CHECK(cudaFreeAsync(tmp, g_stream));
+    BF_CHECK(cudaStreamSynchronize(g_stream));
+    da->parity = sa->parity; da->lastListDual = sa->lastListDual; da->liveValid = sa->liveValid;
+    out[0] = o[0]; out[1] = o[1];
     return 0;
 }
 

@@ -32,7 +32,8 @@ class BFFrameLoopParams(C.Structure):
                 ("maxFrameFixes", C.c_uint32), ("topNActive", C.c_uint32), ("minPoseDistSqrt", C.c_float),
                 ("reconstructionEnabled", C.c_int32),
                 ("hash", BFHashParams),
-                ("renderDepthMin", C.c_float), ("renderDepthMax", C.c_float)]
+                ("renderDepthMin", C.c_float), ("renderDepthMax", C.c_float),
+                ("hashMaxSDFBlocks", C.c_uint32)]
 
 
 class BFFrameLoopStatus(C.Structure):
@@ -67,6 +68,15 @@ class BFFrameLoopFuseInfo(C.Structure):
                 "inserts_dropped": int(self.insertsDropped)}
 
 
+class BFFrameLoopHashGrowth(C.Structure):
+    _fields_ = [("growths", C.c_uint32), ("discarded", C.c_uint32), ("sdfBlocks", C.c_uint32), ("buckets", C.c_uint32), ("maxSDFBlocks", C.c_uint32),
+                ("insertsDropped", C.c_ulonglong), ("ceilingReached", C.c_int32)]
+
+    def as_dict(self):
+        return {"growths": self.growths, "discarded": self.discarded, "sdf_blocks": self.sdfBlocks, "buckets": self.buckets, "max_sdf_blocks": self.maxSDFBlocks,
+                "inserts_dropped": int(self.insertsDropped), "ceiling_reached": bool(self.ceilingReached)}
+
+
 class BFFrameLoopGlobalProblem(C.Structure):
     _fields_ = [("d_correspondences", C.c_void_p), ("numCorrespondences", C.c_uint32), ("numKeyframes", C.c_uint32), ("d_validImages", C.c_void_p),
                 ("d_trajectory", C.c_void_p), ("d_cacheFrames", C.c_void_p), ("cacheWidth", C.c_uint32), ("cacheHeight", C.c_uint32),
@@ -81,6 +91,14 @@ def default_params(width: int, height: int) -> BFFrameLoopParams:
     p = BFFrameLoopParams()
     L.bfFrameLoopDefaultParams(C.byref(p), width, height)
     return p
+
+
+def growth_size(blocks: int, live: int, reserve: int, ceiling: int, init_blocks: int, init_buckets: int) -> tuple:
+    """the loop's growth-size rule (bfFrameLoopHashGrowthSize): (new heap blocks, new bucket count)"""
+    L = _bind(capi.lib())
+    b, k = C.c_uint32(), C.c_uint32()
+    L.bfFrameLoopHashGrowthSize(blocks, live, reserve, ceiling, init_blocks, init_buckets, C.byref(b), C.byref(k))
+    return b.value, k.value
 
 
 def _bind(L):
@@ -105,6 +123,9 @@ def _bind(L):
     L.bfFrameLoopGetHashData.restype = C.POINTER(capi.BFHashDataStruct)
     L.bfFrameLoopGetHashParams.argtypes = [vp]
     L.bfFrameLoopGetHashParams.restype = C.POINTER(BFHashParams)
+    L.bfFrameLoopGetHashGrowth.argtypes = [vp, C.POINTER(BFFrameLoopHashGrowth)]
+    L.bfFrameLoopHashGrowthSize.argtypes = [C.c_uint32, C.c_uint32, C.c_ulonglong, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    L.bfFrameLoopHashGrowthSize.restype = None
     L.bfFrameLoopGetCounters.argtypes = [vp, C.c_ulonglong * 8]
     L.bfFrameLoopGetCounters.restype = None
     L.bfFrameLoopSetOverlap.argtypes = [vp, C.c_int]
@@ -294,6 +315,14 @@ class FrameLoop:
         t = (C.c_double * 8)()
         n = int(self.lib.bfFrameLoopGetStageTimes(self._h, t))
         return {"steps": n, **{k: round(t[i] / max(1, n), 4) for i, k in enumerate(self.STAGES)}}
+
+    def hash_growth(self) -> dict:
+        """growths, current heap and bucket sizes, the ceiling, inserts dropped since creation and whether the ceiling stopped a growth
+        (bfFrameLoopGetHashGrowth; synchronises)"""
+        self._bind_stream()
+        out = BFFrameLoopHashGrowth()
+        capi.check(self.lib.bfFrameLoopGetHashGrowth(self._h, C.byref(out)), "bfFrameLoopGetHashGrowth")
+        return out.as_dict()
 
     def heap_free(self) -> int:
         out = C.c_uint(0)

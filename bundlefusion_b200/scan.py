@@ -7,6 +7,7 @@ the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every 
         [--mesh-voxel-size V]       after the loop, fuse its frames along the final trajectory into a V-sized hash and mesh that (bundlefusion_b200.fuse)
         [--poses recorded]          no loop: fuse along the poses stored with the frames (the reference's s_binaryDumpSensorUseTrajectory)
         [--fit-hash]                size that fused hash from a count of the blocks it will hold (fuse.fit_hash_params), so it drops nothing
+        [--grow-hash MAX_BLOCKS]    start the online hash at --sdf-blocks and let the loop grow it up to MAX_BLOCKS voxel blocks while it scans
 """
 from __future__ import annotations
 
@@ -34,13 +35,15 @@ class _LoopScene:
 
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
                 sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None,
-                mesh_voxel_size: float | None = None, fit_hash: bool = False) -> dict:
+                mesh_voxel_size: float | None = None, fit_hash: bool = False, grow_hash: int | None = None) -> dict:
     """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
     solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
     global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
     None runs a fixed submapSize + 2 past-end turns.  mesh_voxel_size=V: the loop's frames are then fused along its final trajectory into a
     fresh hash of voxel size V (FrameLoop.fuse) and that model is meshed instead of the online one; that call's info goes under "fuse".  With
-    fit_hash that hash is sized by FrameLoop.fit_hash_params, whose report goes under "fit"."""
+    fit_hash that hash is sized by FrameLoop.fit_hash_params, whose report goes under "fit".  grow_hash=MAX_BLOCKS: the online hash starts at
+    sdf_blocks (default: the loop's) and the loop may grow it up to MAX_BLOCKS voxel blocks (hashMaxSDFBlocks); FrameLoop.hash_growth() goes
+    under "hash"."""
     r = SensorDataReader(sens_path)
     n = len(r) if max_frames is None else min(len(r), max_frames)
     P = fuse.recording_params(r.header, n)
@@ -48,6 +51,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
         P.hash.m_hashNumBuckets = hash_buckets
     if sdf_blocks is not None:
         P.hash.m_numSDFBlocks = sdf_blocks
+    if grow_hash is not None:
+        P.hashMaxSDFBlocks = int(grow_hash)
     if tweak is not None:
         tweak(P)
     loop = FrameLoop(P, device)
@@ -71,6 +76,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
            "mesh_path": None, "triangles": 0}
     if finish is not None:
         out["finish"] = finish
+    if grow_hash is not None:
+        out["hash"] = loop.hash_growth()
     if mesh_voxel_size is not None:
         if fit_hash:
             hp, out["fit"] = loop.fit_hash_params(mesh_voxel_size, n=n)
@@ -82,9 +89,10 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
             out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles))
         scene.close()
     elif ply_path is not None:
-        mp = marching_cubes_params(int(P.hash.m_hashNumBuckets), float(P.hash.m_virtualVoxelSize), max_num_triangles)
+        scene = _LoopScene(loop)                       # the table the loop holds now: a grown one has more buckets than P.hash
+        mp = marching_cubes_params(int(scene.m_hashParams.m_hashNumBuckets), float(scene.m_hashParams.m_virtualVoxelSize), max_num_triangles)
         mc = CUDAMarchingCubesHashSDF(mp, device)
-        out["triangles"] = mc.extractIsoSurface(_LoopScene(loop)) // 3
+        out["triangles"] = mc.extractIsoSurface(scene) // 3
         out["mesh_path"] = mc.saveMesh(ply_path, overwrite=True)
         mc.close()
     loop.close(); r.close()
@@ -134,6 +142,9 @@ def main(argv=None) -> int:
     ap.add_argument("--fit-hash", action="store_true",
                     help="with --mesh-voxel-size or --poses recorded: count the blocks the fusion will allocate and size its hash from the count, so that "
                          "no insert is dropped (the JSON summary carries the report under 'fit')")
+    ap.add_argument("--grow-hash", type=int, default=None, metavar="MAX_BLOCKS",
+                    help="start the online hash at --sdf-blocks (default: the loop's) and grow it while scanning, up to MAX_BLOCKS voxel blocks "
+                         "(the JSON summary carries growths, sizes and dropped inserts under 'hash')")
     a = ap.parse_args(argv)
     if a.fit_hash and a.poses != "recorded" and a.mesh_voxel_size is None:
         ap.error("--fit-hash sizes a fused hash: use it with --mesh-voxel-size or --poses recorded")
@@ -150,7 +161,7 @@ def main(argv=None) -> int:
         print(json.dumps(summary))
         return 0
     o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit,
-                    mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash)
+                    mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash, grow_hash=a.grow_hash)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
     summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path")}
@@ -160,6 +171,8 @@ def main(argv=None) -> int:
         summary["fuse"] = {k: o["fuse"][k] for k in ("frames_fused", "frames_skipped", "batches", "inserts_dropped", "heap_free")}
     if "fit" in o:
         summary["fit"] = o["fit"]
+    if "hash" in o:
+        summary["hash"] = {k: o["hash"][k] for k in ("growths", "sdf_blocks", "buckets", "inserts_dropped")}
     gt = recorded_poses(a.sens, a.frames)
     if np.isfinite(gt).all(axis=(1, 2)).sum() >= 3:
         summary["ate"] = ate(o["trajectory"], gt[:len(o["trajectory"])])

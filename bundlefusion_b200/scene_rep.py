@@ -102,7 +102,14 @@ class CUDASceneRepHashSDF:
         self.lib = capi.lib()
         self.m_hashParams = BFHashParams()
         C.memmove(C.byref(self.m_hashParams), C.byref(params), C.sizeof(BFHashParams))
-        hp = self.m_hashParams
+        self.m_hashData = self._allocate(self.m_hashParams)
+        self.m_numIntegratedFrames = 0
+        self.reset()
+
+    # ---- plumbing -----------------------------------------------------------------------
+    def _allocate(self, hp: BFHashParams) -> BFHashDataStruct:
+        """the buffers of a hash of hp's sizes, as HashDataStruct::allocate sizes them (kept alive as attributes of this object)"""
+        torch = self._torch
         n_entries = hp.m_hashNumBuckets * BF_HASH_BUCKET_SIZE
         n_blocks = hp.m_numSDFBlocks
         kw = dict(device=self.device)
@@ -127,11 +134,8 @@ class CUDASceneRepHashSDF:
         hd.d_SDFBlocks = self.d_SDFBlocks.data_ptr()
         hd.d_hashBucketMutex = self.d_hashBucketMutex.data_ptr()
         hd.m_bIsOnGPU = 1
-        self.m_hashData = hd
-        self.m_numIntegratedFrames = 0
-        self.reset()
+        return hd
 
-    # ---- plumbing -----------------------------------------------------------------------
     def _bind_stream(self):
         torch = self._torch
         torch.cuda.set_device(self.device)
@@ -239,6 +243,32 @@ class CUDASceneRepHashSDF:
         self._op_keepalive = (arr, frames)
         capi.check(self.lib.bfTsdfRunOps(C.byref(self.m_hashData), C.byref(self.m_hashParams), C.byref(cam), arr, len(arr), frames[0], frames[1]),
                    "bfTsdfRunOps")
+
+    def rehash(self, num_sdf_blocks: int, num_buckets: int) -> dict:
+        """Move the model into a new table of num_sdf_blocks voxel blocks and num_buckets buckets (bfTsdfRehash): allocate it, reset it, move
+        every live block with its voxels, live-voxel counter and the last compactified list, switch to it and free the old one.  Same block set
+        and voxel words keyed by position; a garbage collection issued next frees what it would have freed before.  Synchronises.  Raises (and
+        keeps the old table) when the new heap cannot hold the live blocks."""
+        self._bind_stream()
+        old_hd, old_hp = self.m_hashData, self.m_hashParams
+        old_bufs = {k: getattr(self, k) for k in ("d_heap", "d_heapCounter", "d_hash", "d_hashDecision", "d_hashDecisionPrefix", "d_hashCompactified",
+                                                   "d_hashCompactifiedCounter", "d_SDFBlocks", "d_hashBucketMutex")}
+        hp = BFHashParams()
+        C.memmove(C.byref(hp), C.byref(old_hp), C.sizeof(BFHashParams))
+        hp.m_numSDFBlocks, hp.m_hashNumBuckets = int(num_sdf_blocks), int(num_buckets)
+        hd = self._allocate(hp)
+        out = (C.c_ulonglong * 2)()
+        rc = self.lib.bfTsdfReset(C.byref(hd), C.byref(hp))
+        if rc == 0:
+            rc = self.lib.bfTsdfRehash(C.byref(old_hd), C.byref(old_hp), C.byref(hd), C.byref(hp), out)
+        if rc != 0:
+            self.lib.bfTsdfReleaseAux(C.byref(hd))
+            for k, v in old_bufs.items():
+                setattr(self, k, v)
+            capi.check(rc, "bfTsdfRehash")
+        self.lib.bfTsdfReleaseAux(C.byref(old_hd))
+        self.m_hashData, self.m_hashParams = hd, hp
+        return {"moved": int(out[0]), "refused": int(out[1])}
 
     def getHashData(self) -> BFHashDataStruct:
         return self.m_hashData

@@ -74,6 +74,7 @@ typedef struct BFFrameLoopParams {
     int32_t  reconstructionEnabled;                                     /* s_reconstructionEnabled (1) */
     BFHashParams hash;                                                  /* voxel hash parameters (poses are set per operation) */
     float    renderDepthMin, renderDepthMax;                            /* frustum test range (0.1, 4.0; SURVEY.md Q4) */
+    uint32_t hashMaxSDFBlocks;                                          /* growth ceiling of the voxel heap (0: a fixed table; see bfFrameLoopGetHashGrowth) */
 } BFFrameLoopParams;
 
 /* fills *p with the defaults of zParametersDefault.txt / zParametersBundlingDefault.txt for a width x height sensor with the synthetic pinhole
@@ -190,9 +191,48 @@ int bfFrameLoopGetKeyframes(const BFFrameLoop* loop, BFKeyframeSet* out);
 
 /* optimised camera-to-world poses of the first n frames (host, [n][16]; invalid frames all -inf); returns the number written */
 unsigned int bfFrameLoopGetTrajectory(BFFrameLoop* loop, float* h_out, unsigned int maxFrames);
-/* the voxel hash the loop integrates into (caller may read it; bf_tsdf.h) */
+/* the voxel hash the loop integrates into (caller may read it; bf_tsdf.h).  With hash growth on, both pointers, and the buffers they name, may
+ * change at a growth: fetch them again after any call that runs a turn (step, past-end turn, bfFrameLoopFinish). */
 const BFHashDataStruct* bfFrameLoopGetHashData(const BFFrameLoop* loop);
 const BFHashParams* bfFrameLoopGetHashParams(const BFFrameLoop* loop);
+
+/* Hash growth.  With hashMaxSDFBlocks > hash.m_numSDFBlocks the loop starts with the table of hash (its bucket and heap sizes) and may move its
+ * model into larger ones, up to hashMaxSDFBlocks voxel blocks; 0 or a value <= hash.m_numSDFBlocks keeps the table fixed (the default).
+ * When: at the start of a turn's reconstruction (steps, past-end turns and bfFrameLoopFinish's turns alike), before its op list runs, decided
+ *   from the free-heap and dropped-insert counters of earlier turns' reconstruction work, which are read back asynchronously (a copy into pinned
+ *   memory and an event, consumed when the event has completed; never waited for).  The loop grows when the free blocks of the last read-back
+ *   fall below a reserve = 2 x the largest one-turn block increase seen so far x the turns since that read-back (>= 1), or when the dropped
+ *   count rose (those inserts are lost: insertsDropped reports them).
+ * Size: new heap = min(hashMaxSDFBlocks, max(2 x old, live + 2 x reserve)); buckets = the initial bucket-to-block ratio (doubled by every
+ *   discarded attempt, below) times the new heap, odd, at most (2^32 - 1) / BF_HASH_BUCKET_SIZE (32-bit entry indices).
+ * How: the reconstruction stream is joined; new buffers are allocated stream-ordered (cudaMallocAsync), bfTsdfReset + bfTsdfRehash move the
+ *   model, the loop switches to the new table and frees the old one stream-ordered (cudaFreeAsync) after releasing its library scratch
+ *   (bfTsdfReleaseAux).  During a growth the old and the new table are both allocated: the peak is their sum.
+ * A new table whose probe windows cannot take every live block (bfTsdfRehash out[1] > 0: the bucket function put too many of them near one
+ *   another) is discarded before the switch: the loop keeps the old table, which the rehash only reads, and tries again with twice the buckets
+ *   per block, at most three attempts per growth; the raised ratio is kept for later growths.  No live block is lost to a growth.
+ * Cost in host synchronisations: a turn that does not grow adds none; each attempt adds BF_FRAMELOOP_GROWTH_SYNCS to bfFrameLoopGetCounters
+ *   out[6] (bfTsdfRehash's read of the source and its completion), so out[6] grows by (growths + discarded) x BF_FRAMELOOP_GROWTH_SYNCS.
+ * The model equals, block for block and word for word keyed by position, the one a fixed table large enough never to drop would hold, as long
+ *   as no insert was dropped (insertsDropped == 0; inserts are dropped when the heap or a probe window of the CURRENT table is full before the
+ *   loop sees it -- the first turn, which runs before any read-back, must fit the initial table).
+ * bfFrameLoopGetHashGrowth joins the reconstruction stream and synchronises (to read the dropped count). */
+#define BF_FRAMELOOP_GROWTH_SYNCS 2
+typedef struct BFFrameLoopHashGrowth {
+    uint32_t growths;                /* tables the model moved into */
+    uint32_t discarded;              /* new tables discarded because they could not take every live block (the old one was kept) */
+    uint32_t sdfBlocks;              /* current heap size (voxel blocks) */
+    uint32_t buckets;                /* current bucket count */
+    uint32_t maxSDFBlocks;           /* the ceiling (hash.m_numSDFBlocks when growth is off) */
+    unsigned long long insertsDropped;   /* block inserts dropped since bfFrameLoopCreate */
+    int32_t  ceilingReached;         /* 1 once a growth was wanted and the ceiling stopped it */
+} BFFrameLoopHashGrowth;
+int bfFrameLoopGetHashGrowth(BFFrameLoop* loop, BFFrameLoopHashGrowth* out);
+/* The growth-size rule alone (no loop): *newBlocks = min(ceiling, max(2 x blocks, live + 2 x reserve)) and *newBuckets = initBuckets x
+ * *newBlocks / initBlocks, made odd, at most (2^32 - 1) / BF_HASH_BUCKET_SIZE.  The loop grows only when *newBlocks > blocks (and never
+ * shrinks the bucket count). */
+void bfFrameLoopHashGrowthSize(uint32_t blocks, uint32_t live, unsigned long long reserve, uint32_t ceiling, uint32_t initBlocks, uint32_t initBuckets,
+                               uint32_t* newBlocks, uint32_t* newBuckets);
 /* Op log (off by default; when off it costs one branch per turn): every BFTsdfOp the loop hands to bfTsdfRunOps -- re-integration items, the
  * GARBAGE_COLLECT, the INTEGRATE of the current frame -- in order, with the turn that issued it (steps and past-end turns, bfFrameLoopFinish's
  * included, counted from 0 since bfFrameLoopCreate).  Enabling it from off starts an empty log; returns the previous setting.

@@ -295,6 +295,26 @@ int bfTsdfBlockKeyMerge(BFBlockKeySet* dst, const BFBlockKeySet* src);
 /* CUDASceneRepHashSDF::garbageCollect (h:110-126) over the last compactified list */
 int bfTsdfGarbageCollect(BFHashDataStruct* hashData, const BFHashParams* hashParams);
 
+/* Move every live block of src into dst, a hash reset by bfTsdfReset with the same voxel size, truncation, truncation scale, maximum
+ * integration distance, block / bucket size, linked-list limit and m_dummy shard setting, and any bucket count and heap size.  Synchronises;
+ * out[0] = blocks moved, out[1] = blocks dst could not take (0 unless dst is too small: its probe window or heap ran out).
+ *
+ * Each live block goes into dst through the insertion rule of every alloc launch (home bucket, else the bucket's overflow list, heap pop, the
+ * slot table), with its voxel words and its live-voxel counter.  The state later calls read moves with it: the live-voxel validity, the dropped-
+ * insert counters (added to dst's, so bfTsdfGetLastFrameStats out[3] still counts every drop since src's reset), the stencil statistics, and
+ * the last compactified list -- same order, same count, its GC flags, each entry's ptr translated to its block's new slot -- so that a
+ * bfTsdfGarbageCollect issued next frees on dst exactly the blocks it would have freed on src.
+ *
+ * The guarantee: two hashes that differ only by a rehash hold the same block set and the same voxel words, keyed by block position, and every
+ * later operation keeps them so.  Heap slots and entry positions may differ, as they already do between two runs of an alloc launch.
+ *
+ * Returns cudaErrorInvalidValue with nothing written to dst for: a NULL argument or buffer, src == dst, any buffer the two share, a differing
+ * parameter of the list above, a bucket count of 0 or above 2^32 / BF_HASH_BUCKET_SIZE, a hash this library does not maintain (not reset by
+ * bfTsdfReset with these sizes), and -- after one synchronising read of src -- a dst heap smaller than src's live blocks or its last list.
+ * Work runs on the library stream; its temporaries are stream-ordered allocations (cudaMallocAsync). */
+int bfTsdfRehash(const BFHashDataStruct* src, const BFHashParams* srcParams, BFHashDataStruct* dst, const BFHashParams* dstParams,
+                 unsigned long long out[2]);
+
 /* synchronising getters (h:168-172 getHeapFreeCount; m_numOccupiedBlocks) */
 int bfTsdfGetHeapFreeCount(const BFHashDataStruct* hashData, unsigned int* outCount);
 int bfTsdfGetNumOccupiedBlocks(const BFHashDataStruct* hashData, unsigned int* outCount);
