@@ -14,6 +14,7 @@
 // + key (the reference packs them by a prefix sum -- which needs each count on the host before the next image can be placed); the chunk ->
 // keyframe fusion and the verification run on the device (csrc/sift_fuse.cu, csrc/sift_verify.cu).
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstring>
 #include <list>
@@ -207,13 +208,39 @@ struct Bundler {
     bool verifyFlag = false;      // SBA::m_bVerify
 };
 
+// ---- the frame store: integration-resolution depth + colour of every frame (CUDAImageManager's frames) -----------------------------------
+// `slots` device slots; frame f's images are in slot slotOf[f] while it is resident.  deviceFrameSlots = 0: one slot per frame, every frame
+// stays where its ingest wrote it.  deviceFrameSlots = N: N slots over a pinned host store of every frame; each ingest is written back to
+// the host on the copy stream, and a frame an op reads is fetched back into a slot (the least recently used one that is not pinned) first.
+// Ordering, never a host wait: a slot is overwritten only after its last reader (evRead, recorded on the stream that read it) and its last
+// copy (evCopy, on the copy stream); a reader waits for the copy that filled the slot.
+struct FrameStore {
+    static const unsigned kChunk = 256;           // frames per pinned host allocation
+    unsigned slots = 0, used = 0;                 // slots are handed out in order until all are used, then reused
+    size_t px = 0;
+    float* d_depth = nullptr; uint8_t* d_color = nullptr;
+    bool spill = false;                           // deviceFrameSlots > 0: the pinned host store exists
+    std::vector<uint8_t*> chunks;                 // host frame f: chunks[f / kChunk] + (f % kChunk) * 8 px, depth then colour
+    cudaStream_t copy = nullptr; cudaEvent_t evIngest = nullptr;
+    std::vector<int> slotOf, frameIn;             // frame -> slot, slot -> frame (-1: none)
+    std::vector<unsigned long long> lastUse;      // slot -> use tick of its last use (LRU victim: the smallest, unpinned)
+    std::vector<char> pin;
+    std::vector<cudaEvent_t> evRead, evCopy;
+    std::vector<int> lent;                        // slots bfFrameLoopFetchFrames handed out: read on the library stream until the next call
+    unsigned long long tick = 0, writeBacks = 0, fetches = 0, hits = 0, evictions = 0, h2d = 0, d2h = 0, hostBytes = 0;
+    double pinMs = 0.0;
+    float* depthOf(int s) const { return d_depth + px * (size_t)s; }
+    uint8_t* colorOf(int s) const { return d_color + px * 4 * (size_t)s; }
+    uint8_t* hostOf(unsigned f) const { return chunks[f / kChunk] + (size_t)(f % kChunk) * px * 8; }
+};
+
 struct Loop {
     BFFrameLoopParams P;
     Arena A;
     // frame input / store
     float* d_depthRaw = nullptr; uint8_t* d_colorRaw = nullptr; float* d_depthFilt = nullptr; float* d_intensity = nullptr;
-    std::vector<float*> d_frameDepth; std::vector<uint8_t*> d_frameColor;      // integration-resolution frame store (CUDAImageManager's frames, kept on the device)
-    std::vector<const float*> depthPtrs; std::vector<const uint8_t*> colorPtrs;
+    FrameStore fs;
+    std::vector<const float*> depthPtrs; std::vector<const uint8_t*> colorPtrs;    // per frame: its slot's images while resident, else NULL
     BFIngestParams ingest, ingestSensorRes; bool needSensorResFilter = false;
     BFSiftDetectParams detect;
     float siftK[16], siftKinv[16];
@@ -285,6 +312,102 @@ static const int PIN_FEAT = 3072;            // h_pin slot the feature stream's 
 static int launch_ahead(Loop& L);
 // every host wait on the library stream: if the next frame's feature work is armed, it is queued first, so that it runs while the host waits
 static int sync_stream(Loop& L) { if (L.aheadArmed) FL_OK(launch_ahead(L)); ++L.counters[6]; BF_CHECK(cudaStreamSynchronize(stream())); return 0; }
+
+// ---- frame store slots ----------------------------------------------------------------------------------------------------------------
+// a slot for frame f (not resident): a never-used one while there are any, else the least recently used unpinned one, whose frame is
+// evicted.  The caller orders the overwrite after the slot's last reader and copy.  Returns -1 when every slot is pinned.
+static int take_slot(Loop& L, unsigned f) {
+    FrameStore& S = L.fs;
+    int s = -1;
+    if (S.used < S.slots) s = (int)S.used++;
+    else
+        for (unsigned k = 0; k < S.slots; ++k)
+            if (!S.pin[k] && (s < 0 || S.lastUse[k] < S.lastUse[s])) s = (int)k;
+    if (s < 0) return -1;
+    const int g = S.frameIn[s];
+    if (g >= 0) { S.slotOf[g] = -1; L.depthPtrs[g] = nullptr; L.colorPtrs[g] = nullptr; ++S.evictions; }
+    S.frameIn[s] = (int)f; S.slotOf[f] = s;
+    L.depthPtrs[f] = S.depthOf(s); L.colorPtrs[f] = S.colorOf(s);
+    return s;
+}
+
+// the slot frame f's ingest writes, on the current stream, pinned until the turn that integrates the frame has fetched its frames
+static int ingest_slot(Loop& L, unsigned f, int* slot) {
+    FrameStore& S = L.fs;
+    const int s = take_slot(L, f);
+    if (s < 0) { set_last_error("frame loop: every frame slot is pinned", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    if (S.spill) { BF_CHECK(cudaStreamWaitEvent(stream(), S.evRead[s], 0)); BF_CHECK(cudaStreamWaitEvent(stream(), S.evCopy[s], 0)); }
+    S.pin[s] = 1; S.lastUse[s] = ++S.tick;
+    *slot = s;
+    return 0;
+}
+
+// after the ingest work of frame f on the current stream (its SIFT detection reads the slot too): the copy stream writes the slot back to the host
+static int write_back(Loop& L, unsigned f) {
+    FrameStore& S = L.fs;
+    if (!S.spill) return 0;
+    const int s = S.slotOf[f];
+    uint8_t* h = S.hostOf(f);
+    BF_CHECK(cudaEventRecord(S.evIngest, stream()));
+    BF_CHECK(cudaStreamWaitEvent(S.copy, S.evIngest, 0));
+    BF_CHECK(cudaMemcpyAsync(h, S.depthOf(s), S.px * 4, cudaMemcpyDeviceToHost, S.copy));
+    BF_CHECK(cudaMemcpyAsync(h + S.px * 4, S.colorOf(s), S.px * 4, cudaMemcpyDeviceToHost, S.copy));
+    BF_CHECK(cudaEventRecord(S.evCopy[s], S.copy));
+    ++S.writeBacks; S.d2h += S.px * 8;
+    return 0;
+}
+
+// Make frames[0, n) resident and pin their slots (one use tick for the group).  A frame without a slot takes one: the copy stream waits for
+// the slot's last reader, copies the frame from the host store and records the slot's copy event; the slot goes into *fetched.  The write-back
+// of the frame was queued on the same copy stream earlier, so the fetch follows it.
+static int fetch_frames(Loop& L, const uint32_t* frames, unsigned n, std::vector<int>* fetched) {
+    FrameStore& S = L.fs;
+    const unsigned long long t = ++S.tick;
+    for (unsigned k = 0; k < n; ++k) {
+        const unsigned f = frames[k];
+        int s = S.slotOf[f];
+        if (s >= 0) { if (S.lastUse[s] != t) ++S.hits; }
+        else {
+            s = take_slot(L, f);
+            if (s < 0) { set_last_error("frame loop: every frame slot is pinned", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+            const uint8_t* h = S.hostOf(f);
+            BF_CHECK(cudaStreamWaitEvent(S.copy, S.evRead[s], 0));
+            BF_CHECK(cudaMemcpyAsync(S.depthOf(s), h, S.px * 4, cudaMemcpyHostToDevice, S.copy));
+            BF_CHECK(cudaMemcpyAsync(S.colorOf(s), h + S.px * 4, S.px * 4, cudaMemcpyHostToDevice, S.copy));
+            BF_CHECK(cudaEventRecord(S.evCopy[s], S.copy));
+            ++S.fetches; S.h2d += S.px * 8;
+            fetched->push_back(s);
+        }
+        S.pin[s] = 1; S.lastUse[s] = t;
+    }
+    return 0;
+}
+
+// the current stream waits for the copies that filled the fetched slots
+static int wait_fetched(Loop& L, const std::vector<int>& fetched) {
+    for (int s : fetched) BF_CHECK(cudaStreamWaitEvent(stream(), L.fs.evCopy[s], 0));
+    return 0;
+}
+
+// frames[0, n) were read by work queued on the current stream: that is their slots' last reader; unpin them
+static int release_frames(Loop& L, const uint32_t* frames, unsigned n) {
+    FrameStore& S = L.fs;
+    for (unsigned k = 0; k < n; ++k) {
+        const int s = S.slotOf[frames[k]];
+        if (s < 0 || !S.pin[s]) continue;
+        if (S.spill) BF_CHECK(cudaEventRecord(S.evRead[s], stream()));
+        S.pin[s] = 0;
+    }
+    return 0;
+}
+
+// at the entry of a call that may reuse slots: the slots the last bfFrameLoopFetchFrames handed out were read on the library stream up to now
+static int settle_lent(Loop& L) {
+    FrameStore& S = L.fs;
+    if (S.spill) for (int s : S.lent) BF_CHECK(cudaEventRecord(S.evRead[s], stream()));
+    S.lent.clear();
+    return 0;
+}
 
 // ---- Bundler::matchAndFilter (FL/Bundler.cpp:103-249) ----------------------------------------------------------------------------------------
 // returns lastMatchedFrame (or -1) in *lastMatched; one host synchronisation at the end (verdict + correspondence count)
@@ -498,8 +621,10 @@ static int front_half(Loop& L, unsigned frame, const float* depth, const uint8_t
     const size_t dB = sizeof(float) * (size_t)P.depthWidth * P.depthHeight, cB = (size_t)4 * P.colorWidth * P.colorHeight;
     BF_CHECK(cudaMemcpyAsync(L.d_depthRaw, depth, dB, onHost ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, stream()));
     BF_CHECK(cudaMemcpyAsync(L.d_colorRaw, color, cB, onHost ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, stream()));
-    FL_OK(bfIngestFrame(&L.ingest, L.d_depthRaw, L.d_colorRaw, L.d_frameDepth[frame], L.d_frameColor[frame]));
-    float* depthFilt = L.d_frameDepth[frame];
+    int slot = -1;
+    FL_OK(ingest_slot(L, frame, &slot));
+    FL_OK(bfIngestFrame(&L.ingest, L.d_depthRaw, L.d_colorRaw, L.fs.depthOf(slot), L.fs.colorOf(slot)));
+    float* depthFilt = L.fs.depthOf(slot);
     if (L.needSensorResFilter) { FL_OK(bfIngestFrame(&L.ingestSensorRes, L.d_depthRaw, L.d_colorRaw, L.d_depthFilt, L.d_colorRaw)); depthFilt = L.d_depthFilt; }
     // getCurrentFrame: intensity at SIFT resolution
     {
@@ -512,7 +637,7 @@ static int front_half(Loop& L, unsigned frame, const float* depth, const uint8_t
     BF_CHECK(cudaMemcpyAsync(h_count, b.sm.d_numKeys + li, sizeof(int), cudaMemcpyDeviceToHost, stream()));
     mark(L, 2);
     FL_OK(b.cache.storeFrame(L.d_depthRaw, L.d_colorRaw));
-    return 0;
+    return write_back(L, frame);
 }
 
 // the front half of the NEXT frame on the feature stream (armed by bfFrameLoopStepAhead once this frame's bookkeeping has fixed the destinations)
@@ -876,11 +1001,17 @@ static int reconstruct(Loop& L, bool gotFrame, unsigned curFrame) {
     if (P.reconstructionEnabled) {
         if (L.opLogOn) { L.opLog.insert(L.opLog.end(), ops.begin(), ops.end()); L.opLogTurn.insert(L.opLogTurn.end(), ops.size(), turn); }
         if (L.grow.on) FL_OK(maybe_grow(L, turn));
+        // the turn's frames into slots (bfTsdfRunOps reads depthPtrs / colorPtrs of these frames only, and not after it returns)
+        std::vector<uint32_t> opFrames; std::vector<int> fetched;
+        for (const BFTsdfOp& op : ops) if (op.kind != BF_TSDF_OP_GARBAGE_COLLECT) opFrames.push_back((uint32_t)op.frame);
+        FL_OK(fetch_frames(L, opFrames.data(), (unsigned)opFrames.size(), &fetched));
         // inputs of this call that live on the main stream: the frame store (ingest of this frame) -- the poses and the op list are host data
         const bool side = L.overlap && !L.profile && L.tsdfStream;
         cudaStream_t mainStream = stream();
         if (side) { BF_CHECK(cudaEventRecord(L.evMain, mainStream)); BF_CHECK(cudaStreamWaitEvent(L.tsdfStream, L.evMain, 0)); bfSetStream(L.tsdfStream); }
-        int rc = bfTsdfRunOps(&L.hd, &L.hp, &L.cam, ops.data(), (int)ops.size(), L.depthPtrs.data(), L.colorPtrs.data());
+        int rc = wait_fetched(L, fetched);
+        if (!rc) rc = bfTsdfRunOps(&L.hd, &L.hp, &L.cam, ops.data(), (int)ops.size(), L.depthPtrs.data(), L.colorPtrs.data());
+        if (!rc) rc = release_frames(L, opFrames.data(), (unsigned)opFrames.size());
         if (!rc && L.grow.on && !L.grow.pending) {              // read back this turn's heap and drop counters behind its work
             rc = tsdf_stats_async(&L.hd, L.grow.h_stat);
             if (!rc) rc = (int)cudaEventRecord(L.grow.ev, stream());
@@ -889,6 +1020,7 @@ static int reconstruct(Loop& L, bool gotFrame, unsigned curFrame) {
         if (side) { cudaEventRecord(L.evTsdf, L.tsdfStream); L.tsdfPending = true; bfSetStream(mainStream); }
         if (rc) return rc;
     }
+    if (gotFrame) { const int s = L.fs.slotOf[curFrame]; if (s >= 0) L.fs.pin[s] = 0; }     // the current frame's pin from its ingest
     return 0;
 }
 // the main stream waits for the reconstruction stream (asynchronously): before anything on it reads the voxel hash, and at the end of a timed region
@@ -921,6 +1053,51 @@ static void release_grown_hash(Loop& L) {
     cudaStreamSynchronize(stream());
     if (L.grow.h_stat) cudaFreeHost(L.grow.h_stat);
     if (L.grow.ev) cudaEventDestroy(L.grow.ev);
+}
+
+// the smallest non-zero deviceFrameSlots: one turn's re-integration frames, the current frame, the announced one, and one fusion batch
+static unsigned min_frame_slots(const BFFrameLoopParams& P) { return std::max(P.maxFrameFixes + 2u, 16u); }
+
+static int frame_store_init(Loop& L) {
+    const BFFrameLoopParams& P = L.P;
+    FrameStore& S = L.fs;
+    S.px = (size_t)P.integrationWidth * P.integrationHeight;
+    S.spill = P.deviceFrameSlots > 0;
+    S.slots = S.spill ? P.deviceFrameSlots : P.maxNumFrames;
+    S.d_depth = L.A.get<float>(S.px * S.slots, false); S.d_color = L.A.get<uint8_t>(S.px * 4 * S.slots, false);
+    if (L.A.err) return L.A.err;
+    S.slotOf.assign(P.maxNumFrames, -1); S.frameIn.assign(S.slots, -1); S.lastUse.assign(S.slots, 0); S.pin.assign(S.slots, 0);
+    L.depthPtrs.assign(P.maxNumFrames, nullptr); L.colorPtrs.assign(P.maxNumFrames, nullptr);
+    if (!S.spill) return 0;
+    BF_CHECK(cudaStreamCreateWithFlags(&S.copy, cudaStreamNonBlocking));
+    BF_CHECK(cudaEventCreateWithFlags(&S.evIngest, cudaEventDisableTiming));
+    S.evRead.assign(S.slots, nullptr); S.evCopy.assign(S.slots, nullptr);
+    for (unsigned s = 0; s < S.slots; ++s) {
+        BF_CHECK(cudaEventCreateWithFlags(&S.evRead[s], cudaEventDisableTiming));
+        BF_CHECK(cudaEventCreateWithFlags(&S.evCopy[s], cudaEventDisableTiming));
+    }
+    // the host store, pinned now: pinning inside a step would stall it
+    const auto t0 = std::chrono::steady_clock::now();
+    for (unsigned f = 0; f < P.maxNumFrames; f += FrameStore::kChunk) {
+        const size_t bytes = (size_t)std::min(FrameStore::kChunk, P.maxNumFrames - f) * S.px * 8;
+        void* p = nullptr;
+        const cudaError_t e = cudaHostAlloc(&p, bytes, cudaHostAllocDefault);
+        if (e != cudaSuccess) { set_last_error("bfFrameLoopCreate: the pinned host frame store", e); cudaGetLastError(); return (int)cudaErrorMemoryAllocation; }
+        S.chunks.push_back(static_cast<uint8_t*>(p)); S.hostBytes += bytes;
+    }
+    S.pinMs = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return 0;
+}
+
+static void frame_store_release(Loop& L) {
+    FrameStore& S = L.fs;
+    if (S.copy) cudaStreamSynchronize(S.copy);
+    for (uint8_t* p : S.chunks) cudaFreeHost(p);
+    for (cudaEvent_t e : S.evRead) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : S.evCopy) if (e) cudaEventDestroy(e);
+    if (S.evIngest) cudaEventDestroy(S.evIngest);
+    if (S.copy) cudaStreamDestroy(S.copy);
+    S.chunks.clear(); S.evRead.clear(); S.evCopy.clear(); S.evIngest = nullptr; S.copy = nullptr;
 }
 
 static void fill_status_tail(Loop& L) {
@@ -971,20 +1148,18 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
     L.P = *params;
     const BFFrameLoopParams& P = L.P;
     if (P.maxNumFrames == 0 || P.submapSize == 0 || P.maxNumImages < 2) { delete Lp; return (int)cudaErrorInvalidValue; }
+    if (P.deviceFrameSlots > 0 && P.deviceFrameSlots < min_frame_slots(P)) {
+        set_last_error("bfFrameLoopCreate: deviceFrameSlots below max(maxFrameFixes + 2, 16)", cudaErrorInvalidValue);
+        delete Lp; return (int)cudaErrorInvalidValue;
+    }
     int rc = 0;
     do {
         L.d_depthRaw = L.A.get<float>((size_t)P.depthWidth * P.depthHeight); L.d_colorRaw = L.A.get<uint8_t>((size_t)P.colorWidth * P.colorHeight * 4);
         L.d_intensity = L.A.get<float>((size_t)P.siftWidth * P.siftHeight);
         L.needSensorResFilter = (P.integrationWidth != P.depthWidth || P.integrationHeight != P.depthHeight);
         if (L.needSensorResFilter) L.d_depthFilt = L.A.get<float>((size_t)P.depthWidth * P.depthHeight);
-        // the device frame store: every frame's integration-resolution depth + colour stays resident for re-integration
-        {
-            const size_t px = (size_t)P.integrationWidth * P.integrationHeight;
-            float* allD = L.A.get<float>(px * P.maxNumFrames, false); uint8_t* allC = L.A.get<uint8_t>(px * 4 * P.maxNumFrames, false);
-            if (L.A.err) { rc = L.A.err; break; }
-            L.d_frameDepth.resize(P.maxNumFrames); L.d_frameColor.resize(P.maxNumFrames); L.depthPtrs.resize(P.maxNumFrames); L.colorPtrs.resize(P.maxNumFrames);
-            for (unsigned f = 0; f < P.maxNumFrames; ++f) { L.d_frameDepth[f] = allD + px * f; L.d_frameColor[f] = allC + px * 4 * f; L.depthPtrs[f] = L.d_frameDepth[f]; L.colorPtrs[f] = L.d_frameColor[f]; }
-        }
+        // the device frame store: one slot per frame (deviceFrameSlots = 0), or deviceFrameSlots slots over a pinned host store of every frame
+        if ((rc = frame_store_init(L))) break;
         memset(&L.ingest, 0, sizeof(L.ingest));
         L.ingest.depthWidth = P.depthWidth; L.ingest.depthHeight = P.depthHeight; L.ingest.colorWidth = P.colorWidth; L.ingest.colorHeight = P.colorHeight;
         L.ingest.widthIntegration = P.integrationWidth; L.ingest.heightIntegration = P.integrationHeight;
@@ -1061,6 +1236,7 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
         if (L.h_pin) cudaFreeHost(L.h_pin);
         if (L.h_complete) cudaFreeHost(L.h_complete);
         if (L.grow.on) release_grown_hash(L);
+        frame_store_release(L);
         delete Lp; return rc;
     }
     *out = reinterpret_cast<BFFrameLoop*>(Lp);
@@ -1075,6 +1251,7 @@ BF_API void bfFrameLoopDestroy(BFFrameLoop* loop) {
     cudaStreamSynchronize(stream());
     bfTsdfReleaseAux(&L->hd);
     if (L->grow.on) release_grown_hash(*L);
+    frame_store_release(*L);
     if (L->tsdfStream) cudaStreamDestroy(L->tsdfStream);
     if (L->featStream) cudaStreamDestroy(L->featStream);
     if (L->evStepStart) cudaEventDestroy(L->evStepStart);
@@ -1119,6 +1296,7 @@ static int ensure_feature_stream(Loop& L) {
 static int step_frame(Loop& L, const float* depth, const uint8_t* color, const float* nextDepth, const uint8_t* nextColor, int onHost, BFFrameLoopStatus* status) {
     const BFFrameLoopParams& P = L.P;
     if (L.numFrames >= P.maxNumFrames) return (int)cudaErrorMemoryAllocation;
+    FL_OK(settle_lent(L));
     const unsigned curFrame = L.numFrames;
     memset(&L.status, 0, sizeof(L.status));
     L.status.frame = curFrame; L.status.localSolved = -1; L.status.lastMatchedFrame = -1;
@@ -1165,6 +1343,7 @@ BF_API int bfFrameLoopStepAhead(BFFrameLoop* loop, const float* depth, const uin
 }
 
 static int past_end_turn(Loop& L, BFFrameLoopStatus* status) {
+    FL_OK(settle_lent(L));
     memset(&L.status, 0, sizeof(L.status));
     L.status.frame = L.numFrames - 1; L.status.localSolved = -1; L.status.lastMatchedFrame = -1;
     process_input_past_end(L);
@@ -1243,32 +1422,43 @@ BF_API int bfFrameLoopFuse(BFFrameLoop* loop, BFHashDataStruct* hd, BFHashParams
         bfTrajectoryGetOptimizedTransforms(L.tm, traj.data());          // frames it has no pose for stay -inf: skipped
         h_poses = traj.data();
     }
+    FL_OK(settle_lent(L));
     FL_OK(join_tsdf(L));
     const bool batch = tsdf_batching_usable() != 0;
     BFFrameLoopFuseInfo fi; memset(&fi, 0, sizeof(fi));
-    int32_t frames[16]; float poses[16 * 16];
+    // the batches: the finite-pose frames in order, <= 16 per batch
+    std::vector<std::vector<uint32_t>> bFrames; std::vector<std::vector<float>> bPoses;
+    for (uint32_t f = 0; f < numFrames; ++f) {
+        const float* T = h_poses + 16 * (size_t)f;
+        bool finite = true;
+        for (int e = 0; e < 16; ++e) finite = finite && std::isfinite(T[e]);
+        if (!finite) { ++fi.framesSkipped; continue; }
+        if (bFrames.empty() || bFrames.back().size() == 16) { bFrames.emplace_back(); bPoses.emplace_back(); }
+        bFrames.back().push_back(f); bPoses.back().insert(bPoses.back().end(), T, T + 16);
+    }
+    // each batch is staged through slots; with room for two batches the next one is fetched while this one integrates
+    const bool prefetch = L.fs.slots >= 32;
+    std::vector<int> fetched[2];
     std::vector<BFTsdfOp> ops;
-    unsigned n = 0;
-    for (uint32_t f = 0; f <= numFrames; ++f) {
-        if (f < numFrames) {
-            const float* T = h_poses + 16 * (size_t)f;
-            bool finite = true;
-            for (int e = 0; e < 16; ++e) finite = finite && std::isfinite(T[e]);
-            if (!finite) { ++fi.framesSkipped; continue; }
-            frames[n] = (int32_t)f; memcpy(poses + 16 * n, T, 64); ++n;
-            if (n < 16) continue;
-        }
-        if (n == 0) continue;
+    for (size_t b = 0; b < bFrames.size(); ++b) {
+        const std::vector<uint32_t>& fr = bFrames[b];
+        const unsigned n = (unsigned)fr.size();
+        if (b == 0 || !prefetch) FL_OK(fetch_frames(L, fr.data(), n, &fetched[b & 1]));
+        if (prefetch && b + 1 < bFrames.size()) FL_OK(fetch_frames(L, bFrames[b + 1].data(), (unsigned)bFrames[b + 1].size(), &fetched[(b + 1) & 1]));
+        FL_OK(wait_fetched(L, fetched[b & 1]));
+        fetched[b & 1].clear();
         if (batch) {
-            FL_OK(bfTsdfIntegrateBatch(hd, hp, &L.cam, frames, poses, (int)n, L.depthPtrs.data(), L.colorPtrs.data()));
+            const std::vector<int32_t> frames(fr.begin(), fr.end());
+            FL_OK(bfTsdfIntegrateBatch(hd, hp, &L.cam, frames.data(), bPoses[b].data(), (int)n, L.depthPtrs.data(), L.colorPtrs.data()));
             FL_OK(bfTsdfGarbageCollect(hd, hp));
         } else {
             ops.assign(n + 1, BFTsdfOp{});
-            for (unsigned k = 0; k < n; ++k) { ops[k].kind = BF_TSDF_OP_INTEGRATE; ops[k].frame = frames[k]; memcpy(ops[k].pose, poses + 16 * k, 64); }
+            for (unsigned k = 0; k < n; ++k) { ops[k].kind = BF_TSDF_OP_INTEGRATE; ops[k].frame = (int32_t)fr[k]; memcpy(ops[k].pose, bPoses[b].data() + 16 * k, 64); }
             ops[n].kind = BF_TSDF_OP_GARBAGE_COLLECT;
             FL_OK(bfTsdfRunOps(hd, hp, &L.cam, ops.data(), (int)ops.size(), L.depthPtrs.data(), L.colorPtrs.data()));
         }
-        fi.framesFused += n; ++fi.batches; n = 0;
+        FL_OK(release_frames(L, fr.data(), n));
+        fi.framesFused += n; ++fi.batches;
     }
     unsigned long long st[4] = { 0, 0, 0, 0 };
     if (fi.batches) FL_OK(bfTsdfGetLastFrameStats(hd, st));
@@ -1334,11 +1524,43 @@ BF_API uint32_t bfFrameLoopGetOpLog(const BFFrameLoop* loop, BFTsdfOp* out, uint
     if (turnOfOp) std::copy(L.opLogTurn.begin(), L.opLogTurn.begin() + m, turnOfOp);
     return (uint32_t)L.opLog.size();
 }
+BF_API int bfFrameLoopFetchFrames(BFFrameLoop* loop, const uint32_t* frames, uint32_t n, const float** depth, const uint8_t** color) {
+    if (!loop || !frames || !depth || !color) return (int)cudaErrorInvalidValue;
+    Loop& L = *reinterpret_cast<Loop*>(loop);
+    if ((unsigned long long)n + 2 > L.fs.slots) { set_last_error("bfFrameLoopFetchFrames: more than deviceFrameSlots - 2 frames", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    for (uint32_t k = 0; k < n; ++k)
+        if (frames[k] >= L.numFrames) { set_last_error("bfFrameLoopFetchFrames: a frame has not been stepped", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
+    FL_OK(settle_lent(L));
+    FL_OK(join_tsdf(L));                    // every earlier reader of a slot is on the library stream: its next read event covers them all
+    std::vector<int> fetched;
+    FL_OK(fetch_frames(L, frames, n, &fetched));
+    FL_OK(wait_fetched(L, fetched));
+    for (uint32_t k = 0; k < n; ++k) {
+        depth[k] = L.depthPtrs[frames[k]]; color[k] = L.colorPtrs[frames[k]];
+        const int s = L.fs.slotOf[frames[k]];
+        if (L.fs.pin[s]) { L.fs.pin[s] = 0; L.fs.lent.push_back(s); }
+    }
+    return 0;
+}
 BF_API int bfFrameLoopGetFrame(const BFFrameLoop* loop, uint32_t f, const float** depth, const uint8_t** color) {
     if (!loop || !depth || !color) return (int)cudaErrorInvalidValue;
     const Loop& L = *reinterpret_cast<const Loop*>(loop);
     if (f >= L.numFrames) { set_last_error("bfFrameLoopGetFrame: the frame has not been stepped", cudaErrorInvalidValue); return (int)cudaErrorInvalidValue; }
-    *depth = L.d_frameDepth[f]; *color = L.d_frameColor[f];
+    if (L.fs.spill) return bfFrameLoopFetchFrames(const_cast<BFFrameLoop*>(loop), &f, 1, depth, color);
+    *depth = L.depthPtrs[f]; *color = L.colorPtrs[f];
+    return 0;
+}
+BF_API int bfFrameLoopGetFrameStore(const BFFrameLoop* loop, BFFrameLoopFrameStore* out) {
+    if (!loop || !out) return (int)cudaErrorInvalidValue;
+    const FrameStore& S = reinterpret_cast<const Loop*>(loop)->fs;
+    memset(out, 0, sizeof(*out));
+    out->slots = S.slots; out->hostStore = S.spill ? 1 : 0;
+    unsigned resident = 0;
+    for (int f : S.frameIn) resident += f >= 0 ? 1u : 0u;
+    out->residentFrames = resident;
+    out->deviceBytes = (unsigned long long)S.slots * S.px * 8; out->hostBytes = S.hostBytes;
+    out->writeBacks = S.writeBacks; out->fetches = S.fetches; out->hits = S.hits; out->evictions = S.evictions;
+    out->h2dBytes = S.h2d; out->d2hBytes = S.d2h; out->pinMs = S.pinMs;
     return 0;
 }
 BF_API int bfFrameLoopJoin(BFFrameLoop* loop) { return loop ? join_tsdf(*reinterpret_cast<Loop*>(loop)) : (int)cudaErrorInvalidValue; }

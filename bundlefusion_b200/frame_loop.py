@@ -33,7 +33,7 @@ class BFFrameLoopParams(C.Structure):
                 ("reconstructionEnabled", C.c_int32),
                 ("hash", BFHashParams),
                 ("renderDepthMin", C.c_float), ("renderDepthMax", C.c_float),
-                ("hashMaxSDFBlocks", C.c_uint32)]
+                ("hashMaxSDFBlocks", C.c_uint32), ("deviceFrameSlots", C.c_uint32)]
 
 
 class BFFrameLoopStatus(C.Structure):
@@ -75,6 +75,17 @@ class BFFrameLoopHashGrowth(C.Structure):
     def as_dict(self):
         return {"growths": self.growths, "discarded": self.discarded, "sdf_blocks": self.sdfBlocks, "buckets": self.buckets, "max_sdf_blocks": self.maxSDFBlocks,
                 "inserts_dropped": int(self.insertsDropped), "ceiling_reached": bool(self.ceilingReached)}
+
+
+class BFFrameLoopFrameStore(C.Structure):
+    _fields_ = [("slots", C.c_uint32), ("hostStore", C.c_int32), ("residentFrames", C.c_uint32), ("deviceBytes", C.c_ulonglong), ("hostBytes", C.c_ulonglong),
+                ("writeBacks", C.c_ulonglong), ("fetches", C.c_ulonglong), ("hits", C.c_ulonglong), ("evictions", C.c_ulonglong),
+                ("h2dBytes", C.c_ulonglong), ("d2hBytes", C.c_ulonglong), ("pinMs", C.c_double)]
+
+    def as_dict(self):
+        return {"slots": self.slots, "host_store": bool(self.hostStore), "resident_frames": self.residentFrames, "device_bytes": int(self.deviceBytes),
+                "host_bytes": int(self.hostBytes), "write_backs": int(self.writeBacks), "fetches": int(self.fetches), "hits": int(self.hits),
+                "evictions": int(self.evictions), "h2d_bytes": int(self.h2dBytes), "d2h_bytes": int(self.d2hBytes), "pin_ms": float(self.pinMs)}
 
 
 class BFFrameLoopGlobalProblem(C.Structure):
@@ -134,6 +145,8 @@ def _bind(L):
     L.bfFrameLoopGetOpLog.argtypes = [vp, C.POINTER(capi.BFTsdfOp), C.POINTER(C.c_uint32), C.c_uint32]
     L.bfFrameLoopGetOpLog.restype = C.c_uint32
     L.bfFrameLoopGetFrame.argtypes = [vp, C.c_uint32, C.POINTER(vp), C.POINTER(vp)]
+    L.bfFrameLoopFetchFrames.argtypes = [vp, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(vp), C.POINTER(vp)]
+    L.bfFrameLoopGetFrameStore.argtypes = [vp, C.POINTER(BFFrameLoopFrameStore)]
     L.bfFrameLoopSetProfiling.argtypes = [vp, C.c_int]
     L.bfFrameLoopGetStageTimes.argtypes = [vp, C.c_double * 8]
     L.bfFrameLoopGetStageTimes.restype = C.c_ulonglong
@@ -240,12 +253,12 @@ class FrameLoop:
         C.memmove(C.byref(hp), C.byref(self.params.hash), C.sizeof(BFHashParams))
         hp.m_virtualVoxelSize = voxel_size
         counter = fuse.BlockCounter(hp, self.device)
-        depth = []
-        for f in fin:
-            d, c = C.c_void_p(), C.c_void_p()
-            capi.check(self.lib.bfFrameLoopGetFrame(self._h, int(f), C.byref(d), C.byref(c)), "bfFrameLoopGetFrame")
-            depth.append(d.value)
-        counter.add(depth, T[fin], fuse.integration_camera(self.params))
+        cam = fuse.integration_camera(self.params)
+        g = max(1, min(8, self.frame_store()["slots"] - 2))
+        for s in range(0, len(fin), g):                # fetched frames' pointers hold until the next loop call: count them before it
+            group = fin[s:s + g]
+            depth, _ = self.fetch_frames(group)
+            counter.add(depth, T[group], cam)
         return fuse.fit_hash_params(self.params.hash, voxel_size, counter, max_table_bytes)
 
     def global_problem(self) -> BFFrameLoopGlobalProblem:
@@ -294,18 +307,39 @@ class FrameLoop:
         words = raw.view(np.int32)
         return words[:, 0].copy(), words[:, 1].copy(), raw[:, 8:].copy().view(np.float32).reshape(m, 4, 4), turns[:m].copy()
 
-    def frame(self, f: int):
-        """frame f as the loop's frame store holds it (bfFrameLoopGetFrame): (depth float32 [H, W], colour uint8 [H, W, 4]) torch views of the
-        loop's device memory at integration resolution -- no copy, valid while the loop lives"""
-        d, c = C.c_void_p(), C.c_void_p()
-        capi.check(self.lib.bfFrameLoopGetFrame(self._h, int(f), C.byref(d), C.byref(c)), "bfFrameLoopGetFrame")
+    def _views(self, d, c):
         W, H = int(self.params.integrationWidth), int(self.params.integrationHeight)
 
         class _View:
             def __init__(self, ptr, shape, typestr):
                 self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "version": 3, "strides": None}
         t = self._torch
-        return (t.as_tensor(_View(d.value, (H, W), "<f4"), device=self.device), t.as_tensor(_View(c.value, (H, W, 4), "|u1"), device=self.device))
+        return (t.as_tensor(_View(d, (H, W), "<f4"), device=self.device), t.as_tensor(_View(c, (H, W, 4), "|u1"), device=self.device))
+
+    def frame(self, f: int):
+        """frame f as the loop's frame store holds it (bfFrameLoopGetFrame): (depth float32 [H, W], colour uint8 [H, W, 4]) torch views of the
+        loop's device memory at integration resolution, no copy.  With deviceFrameSlots = 0 they are valid while the loop lives.  With device
+        frame slots the frame is fetched into a slot (bfFrameLoopFetchFrames) and the views are valid until the next call on the loop: read them
+        on the current stream before it, or clone them."""
+        self._bind_stream()
+        d, c = C.c_void_p(), C.c_void_p()
+        capi.check(self.lib.bfFrameLoopGetFrame(self._h, int(f), C.byref(d), C.byref(c)), "bfFrameLoopGetFrame")
+        return self._views(d.value, c.value)
+
+    def fetch_frames(self, frames):
+        """frames (at most slots - 2) made resident in the frame store (bfFrameLoopFetchFrames): (depth pointers, colour pointers), device
+        addresses valid until the next call on the loop; the current stream is ordered after the copies"""
+        self._bind_stream()
+        f = np.ascontiguousarray(frames, dtype=np.uint32).reshape(-1)
+        d, c = (C.c_void_p * max(1, len(f)))(), (C.c_void_p * max(1, len(f)))()
+        capi.check(self.lib.bfFrameLoopFetchFrames(self._h, f.ctypes.data_as(C.POINTER(C.c_uint32)), len(f), d, c), "bfFrameLoopFetchFrames")
+        return [int(x or 0) for x in d[:len(f)]], [int(x or 0) for x in c[:len(f)]]
+
+    def frame_store(self) -> dict:
+        """slots, device and pinned host bytes, write-backs, fetches, hits, evictions and copy bytes of the frame store (bfFrameLoopGetFrameStore)"""
+        out = BFFrameLoopFrameStore()
+        capi.check(self.lib.bfFrameLoopGetFrameStore(self._h, C.byref(out)), "bfFrameLoopGetFrameStore")
+        return out.as_dict()
 
     def set_profiling(self, enable: bool) -> None:
         capi.check(self.lib.bfFrameLoopSetProfiling(self._h, 1 if enable else 0), "bfFrameLoopSetProfiling")

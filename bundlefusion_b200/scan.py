@@ -8,6 +8,7 @@ the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every 
         [--poses recorded]          no loop: fuse along the poses stored with the frames (the reference's s_binaryDumpSensorUseTrajectory)
         [--fit-hash]                size that fused hash from a count of the blocks it will hold (fuse.fit_hash_params), so it drops nothing
         [--grow-hash MAX_BLOCKS]    start the online hash at --sdf-blocks and let the loop grow it up to MAX_BLOCKS voxel blocks while it scans
+        [--device-frames N]         keep N frame slots on the device and every frame in pinned host memory (same results, less device memory)
 """
 from __future__ import annotations
 
@@ -35,7 +36,8 @@ class _LoopScene:
 
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
                 sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None,
-                mesh_voxel_size: float | None = None, fit_hash: bool = False, grow_hash: int | None = None) -> dict:
+                mesh_voxel_size: float | None = None, fit_hash: bool = False, grow_hash: int | None = None,
+                device_frames: int | None = None) -> dict:
     """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
     solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
     global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
@@ -43,7 +45,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
     fresh hash of voxel size V (FrameLoop.fuse) and that model is meshed instead of the online one; that call's info goes under "fuse".  With
     fit_hash that hash is sized by FrameLoop.fit_hash_params, whose report goes under "fit".  grow_hash=MAX_BLOCKS: the online hash starts at
     sdf_blocks (default: the loop's) and the loop may grow it up to MAX_BLOCKS voxel blocks (hashMaxSDFBlocks); FrameLoop.hash_growth() goes
-    under "hash"."""
+    under "hash".  device_frames=N keeps N frame slots on the device over a pinned host store of every frame (deviceFrameSlots); the results
+    do not change, and FrameLoop.frame_store() goes under "frame_store"."""
     r = SensorDataReader(sens_path)
     n = len(r) if max_frames is None else min(len(r), max_frames)
     P = fuse.recording_params(r.header, n)
@@ -53,6 +56,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
         P.hash.m_numSDFBlocks = sdf_blocks
     if grow_hash is not None:
         P.hashMaxSDFBlocks = int(grow_hash)
+    if device_frames is not None:
+        P.deviceFrameSlots = int(device_frames)
     if tweak is not None:
         tweak(P)
     loop = FrameLoop(P, device)
@@ -95,6 +100,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
         out["triangles"] = mc.extractIsoSurface(scene) // 3
         out["mesh_path"] = mc.saveMesh(ply_path, overwrite=True)
         mc.close()
+    if device_frames is not None:
+        out["frame_store"] = loop.frame_store()
     loop.close(); r.close()
     return out
 
@@ -145,6 +152,9 @@ def main(argv=None) -> int:
     ap.add_argument("--grow-hash", type=int, default=None, metavar="MAX_BLOCKS",
                     help="start the online hash at --sdf-blocks (default: the loop's) and grow it while scanning, up to MAX_BLOCKS voxel blocks "
                          "(the JSON summary carries growths, sizes and dropped inserts under 'hash')")
+    ap.add_argument("--device-frames", type=int, default=None, metavar="N",
+                    help="keep N frame slots on the device over a pinned host store of every frame, N >= 16 (the results do not change; the JSON "
+                         "summary carries slots, bytes, fetches and hits under 'frame_store')")
     a = ap.parse_args(argv)
     if a.fit_hash and a.poses != "recorded" and a.mesh_voxel_size is None:
         ap.error("--fit-hash sizes a fused hash: use it with --mesh-voxel-size or --poses recorded")
@@ -161,7 +171,8 @@ def main(argv=None) -> int:
         print(json.dumps(summary))
         return 0
     o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit,
-                    mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash, grow_hash=a.grow_hash)
+                    mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash, grow_hash=a.grow_hash,
+                    device_frames=a.device_frames)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
     summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path")}
@@ -173,6 +184,8 @@ def main(argv=None) -> int:
         summary["fit"] = o["fit"]
     if "hash" in o:
         summary["hash"] = {k: o["hash"][k] for k in ("growths", "sdf_blocks", "buckets", "inserts_dropped")}
+    if "frame_store" in o:
+        summary["frame_store"] = o["frame_store"]
     gt = recorded_poses(a.sens, a.frames)
     if np.isfinite(gt).all(axis=(1, 2)).sum() >= 3:
         summary["ate"] = ate(o["trajectory"], gt[:len(o["trajectory"])])

@@ -75,6 +75,7 @@ typedef struct BFFrameLoopParams {
     BFHashParams hash;                                                  /* voxel hash parameters (poses are set per operation) */
     float    renderDepthMin, renderDepthMax;                            /* frustum test range (0.1, 4.0; SURVEY.md Q4) */
     uint32_t hashMaxSDFBlocks;                                          /* growth ceiling of the voxel heap (0: a fixed table; see bfFrameLoopGetHashGrowth) */
+    uint32_t deviceFrameSlots;                                          /* device frame slots over a pinned host frame store (0: every frame on the device; see bfFrameLoopGetFrameStore) */
 } BFFrameLoopParams;
 
 /* fills *p with the defaults of zParametersDefault.txt / zParametersBundlingDefault.txt for a width x height sensor with the synthetic pinhole
@@ -101,7 +102,8 @@ typedef struct BFFrameLoopStatus {
 
 typedef struct BFFrameLoop BFFrameLoop;
 
-/* allocates every device buffer of the loop (frame store, SIFT managers, caches, solvers, trajectories, voxel hash); returns 0 or a cudaError_t */
+/* allocates every device buffer of the loop (frame store, SIFT managers, caches, solvers, trajectories, voxel hash) and, with deviceFrameSlots > 0,
+ * the pinned host frame store (bfFrameLoopFetchFrames); returns 0 or a cudaError_t */
 int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out);
 void bfFrameLoopDestroy(BFFrameLoop* loop);
 
@@ -240,8 +242,47 @@ void bfFrameLoopHashGrowthSize(uint32_t blocks, uint32_t live, unsigned long lon
 int bfFrameLoopSetOpLog(BFFrameLoop* loop, int enable);
 uint32_t bfFrameLoopGetOpLog(const BFFrameLoop* loop, BFTsdfOp* out, uint32_t* turnOfOp, uint32_t maxOps);
 /* Device pointers into the loop's frame store: the integration-resolution depth (float [integrationHeight][integrationWidth]) and colour
- * (uchar4) of frame f, the images every TSDF op of frame f reads.  Written on the library stream; cudaErrorInvalidValue for a frame not yet stepped. */
+ * (uchar4) of frame f, the images every TSDF op of frame f reads.  Written on the library stream; cudaErrorInvalidValue for a frame not yet stepped.
+ * With deviceFrameSlots = 0 the pointers stay valid while the loop lives.  With deviceFrameSlots > 0 this is bfFrameLoopFetchFrames(loop, &f, 1, ...)
+ * and its lifetime applies. */
 int bfFrameLoopGetFrame(const BFFrameLoop* loop, uint32_t f, const float** depth, const uint8_t** color);
+
+/* The frame store.
+ * deviceFrameSlots = 0 (the default): every frame has its own device slot, allocated at bfFrameLoopCreate (maxNumFrames x integrationWidth x
+ *   integrationHeight x 8 bytes).
+ * deviceFrameSlots = N > 0: the device holds N slots (N x W x H x 8 bytes); every frame also lives in a pinned host store of maxNumFrames frames,
+ *   pinned at create in chunks of 256 frames (a chunk that cannot be pinned fails the create with cudaErrorMemoryAllocation).  N must be at
+ *   least max(maxFrameFixes + 2, 16) -- one turn's re-integration frames, the current frame, the frame announced by bfFrameLoopStepAhead, and
+ *   one fusion batch of 16 -- else the create returns cudaErrorInvalidValue.
+ *   - After a frame's ingest writes its slot, the loop's copy stream copies the slot to the host store (write-back).
+ *   - Before a turn's op list, a fusion batch of bfFrameLoopFuse or a bfFrameLoopFetchFrames call, each of its frames without a slot takes one
+ *     and is copied in from the host store (fetch).  The victim is the least recently used slot that is not pinned; the frames of the current
+ *     turn or batch, the current frame and the announced frame are pinned.  bfFrameLoopFuse with N >= 32 fetches batch b + 1 while batch b
+ *     integrates; below 32 fetch and integrate alternate.
+ *   - Ordering is by events between streams only, never a host wait: a copy into a slot waits for the slot's last reader (an event on the
+ *     stream that read it), and the stream that reads a fetched frame waits for its copy.
+ * Results do not depend on N: the same ops run in the same order on the same bytes, only the addresses differ.  Statuses, trajectory, op log,
+ * model, bfFrameLoopFinish / bfFrameLoopFuse results and bfFrameLoopGetCounters (host synchronisations included) equal those of
+ * deviceFrameSlots = 0.
+ *
+ * bfFrameLoopFetchFrames makes frames[0, n) resident and writes their slots' device pointers to depth[k] / color[k]; the library stream is ordered
+ * after the copies (no host wait).  n <= slots - 2, every frame stepped, else cudaErrorInvalidValue with nothing enqueued.  The pointers are
+ * valid until the next bfFrameLoop* call on the loop: work that reads them must be queued on the library stream before that call. */
+int bfFrameLoopFetchFrames(BFFrameLoop* loop, const uint32_t* frames, uint32_t n, const float** depth, const uint8_t** color);
+typedef struct BFFrameLoopFrameStore {
+    uint32_t slots;                      /* device frame slots (maxNumFrames when deviceFrameSlots = 0) */
+    int32_t  hostStore;                  /* 1: a pinned host store backs the slots */
+    uint32_t residentFrames;             /* frames in a slot now */
+    unsigned long long deviceBytes;      /* slots x W x H x 8 */
+    unsigned long long hostBytes;        /* pinned host store */
+    unsigned long long writeBacks;       /* frames copied to the host store */
+    unsigned long long fetches;          /* frames copied into a slot from the host store */
+    unsigned long long hits;             /* frames of an op list, fusion batch or fetch call that were already in a slot */
+    unsigned long long evictions;        /* frames whose slot was given to another frame */
+    unsigned long long h2dBytes, d2hBytes;
+    double   pinMs;                      /* host time bfFrameLoopCreate spent pinning the host store */
+} BFFrameLoopFrameStore;
+int bfFrameLoopGetFrameStore(const BFFrameLoop* loop, BFFrameLoopFrameStore* out);
 /* counters for measurement: out[0] frames, out[1] integrations, out[2] re-integrations, out[3] local solves, out[4] global solves,
  * out[5] PCG iterations (global, last solve), out[6] host synchronisations, out[7] keyframes */
 void bfFrameLoopGetCounters(const BFFrameLoop* loop, unsigned long long out[8]);
