@@ -136,7 +136,9 @@ class BFRayCastData(C.Structure):
 
 MARCHINGCUBES_SYMBOLS = ["resetMarchingCubesCUDA", "extractIsoSurfaceCUDA", "bfMarchingCubesExtract", "bfMarchingCubesCreate", "bfMarchingCubesDestroy",
                          "bfMarchingCubesExtractIsoSurface", "bfMarchingCubesClearMeshBuffer", "bfMarchingCubesGetSoup", "bfMarchingCubesSaveMesh",
-                         "bfMeshMergeCloseVertices", "bfMeshRemoveDuplicateFaces", "bfMeshSavePly"]
+                         "bfMeshMergeCloseVertices", "bfMeshRemoveDuplicateFaces", "bfMeshSavePly", "bfMarchingCubesCount", "bfMarchingCubesExtractRange",
+                         "bfMarchingCubesExtractIsoSurfaceWhole", "bfMarchingCubesGetLastExtraction"]
+BF_MC_CHUNK_SLOTS = 512                  # hash slots per chunk of the count pass and of bfMarchingCubesExtractRange
 
 
 class BFMarchingCubesParams(C.Structure):
@@ -149,6 +151,12 @@ class BFMarchingCubesParams(C.Structure):
 class BFMarchingCubesData(C.Structure):
     """include/bf_marchingcubes.h (FL/DepthSensing/MarchingCubesSDFUtil.h:281-286)"""
     _fields_ = [("d_params", C.c_void_p), ("d_numTriangles", C.c_void_p), ("d_triangles", C.c_void_p), ("m_bIsOnGPU", C.c_uint8)]
+
+
+class BFMarchingCubesWholeInfo(C.Structure):
+    """include/bf_marchingcubes.h: what bfMarchingCubesExtractIsoSurfaceWhole did, 40 bytes"""
+    _fields_ = [("trianglesCounted", C.c_uint64), ("trianglesExtracted", C.c_uint64), ("chunks", C.c_uint32), ("parts", C.c_uint32),
+                ("largestPart", C.c_uint32), ("bufferTriangles", C.c_uint32), ("bufferEnlarged", C.c_uint32), ("hostSyncs", C.c_uint32)]
 
 
 CACHE_SYMBOLS = ["bfCacheStoreFrame"]

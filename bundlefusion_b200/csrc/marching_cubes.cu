@@ -16,6 +16,9 @@
 //     in shared memory; every sample then reads shared memory.  Values and arithmetic are the reference's (same voxel index rounding, same weights, same order);
 //   * triangles are appended with one global atomicAdd per block instead of one per triangle: cells count their triangles, the CTA reserves a contiguous range.
 //     (The reference's soup order is whatever its atomics produce; so is the order of the blocks here.)
+//   * the same kernel, instantiated with kCount, is a count pass: per 512-slot chunk, the triangles its blocks' cells produce, with no global atomic.  The
+//     extraction can be limited to a chunk range, so the whole-mesh call cuts the table into parts whose triangles fit the buffer (the reference: one
+//     fixed buffer, the rest dropped).
 // Arithmetic contract (bit-exact with oracle/marchingcubes_oracle.c): TU built -fmad=false -prec-div=true, expressions in the reference's order.
 #include <algorithm>
 #include <cmath>
@@ -39,11 +42,14 @@ const BFHashParams* bound_hash_params();                 // tsdf.cu: what update
 
 #define BF_MC_THREADS 512
 #define BF_MC_TILE 10                                    // a block and its one-voxel shell
+static_assert(BF_MC_CHUNK_SLOTS == BF_MC_THREADS, "a chunk of the count pass and of the range extraction is the table slice one CTA takes");
 
 struct McArgs {
     BFHashDataStruct hd; BFHashParams hp; BFMarchingCubesParams p;
     const BFMarchingCubesParams* d_params;               // non-NULL: the cell parameters are read from the device copy (the reference-named stub)
     BFMarchingCubesTriangle* tri; unsigned* count;
+    unsigned chunkBegin, chunkEnd;                       // the 512-slot chunks of the table whose blocks this launch meshes
+    unsigned* chunkCounts;                               // count pass: triangles per chunk
 };
 
 struct McTile { const unsigned* w; I3 origin; };         // staged voxels (3 words each) and the voxel position of tile entry (0, 0, 0)
@@ -82,21 +88,25 @@ __device__ __forceinline__ F3 mc_corner(F3 c, float P, int v) {
     return F3{ c.x + (px ? P : M), c.y + (py ? P : M), c.z + (pz ? P : M) };
 }
 
+// kCount = false: extraction -- each block's triangles go to one contiguous range of a.tri, reserved with one global atomicAdd.
+// kCount = true: the count pass -- the same cell tests, no triangle written and no global atomic; a.chunkCounts[chunk] = the chunk's triangles,
+// a plain store of a CTA-local sum (one CTA owns a chunk), so the counts do not depend on scheduling.
+template <bool kCount>
 __global__ void __launch_bounds__(BF_MC_THREADS)
 mc_extract_kernel(const __grid_constant__ McArgs a) {
     __shared__ unsigned sTile[BF_MC_TILE * BF_MC_TILE * BF_MC_TILE * 3];
     __shared__ unsigned long long sTri[256];
     __shared__ unsigned sOcc[BF_MC_THREADS];
     __shared__ int sPtr[27];
-    __shared__ unsigned sNumOcc, sTotal, sBase;
+    __shared__ unsigned sNumOcc, sTotal, sBase, sChunk;
     const unsigned tid = threadIdx.x;
     if (tid < 256) sTri[tid] = kMcTriangles[tid];
     const BFMarchingCubesParams P = a.d_params ? *a.d_params : a.p;
     const unsigned total = a.hp.m_hashNumBuckets * BF_HASH_BUCKET_SIZE;
     const float vs = a.hp.m_virtualVoxelSize, half = vs / 2.0f;
     const float isolevel = 0.0f;
-    for (unsigned chunk = blockIdx.x; (size_t)chunk * BF_MC_THREADS < total; chunk += gridDim.x) {
-        if (tid == 0) sNumOcc = 0;
+    for (unsigned chunk = a.chunkBegin + blockIdx.x; chunk < a.chunkEnd; chunk += gridDim.x) {
+        if (tid == 0) { sNumOcc = 0; sChunk = 0; }
         __syncthreads();
         const unsigned e = chunk * BF_MC_THREADS + tid;
         if (e < total && __ldg(&a.hd.d_hash[e].ptr) != BF_FREE_ENTRY) sOcc[atomicAdd(&sNumOcc, 1u)] = e;
@@ -163,13 +173,13 @@ mc_extract_kernel(const __grid_constant__ McArgs a) {
             if (live) {
                 const unsigned long long row = sTri[cube];
                 while (nTri < 5u && ((row >> (12u * nTri)) & 15ull) != 15ull) ++nTri;
-                cellColor = mc_voxel(tile, a.hd, a.hp, worldPos, bc).color;                                               // Voxel v = hashData.getVoxel(worldPos)
-                off = atomicAdd(&sTotal, nTri);
+                if (!kCount) cellColor = mc_voxel(tile, a.hd, a.hp, worldPos, bc).color;                                  // Voxel v = hashData.getVoxel(worldPos)
+                if (kCount) atomicAdd(&sChunk, nTri); else off = atomicAdd(&sTotal, nTri);
             }
             __syncthreads();
-            if (tid == 0 && sTotal != 0u) sBase = atomicAdd(a.count, sTotal);
+            if (!kCount && tid == 0 && sTotal != 0u) sBase = atomicAdd(a.count, sTotal);
             __syncthreads();
-            if (nTri != 0u) {
+            if (!kCount && nTri != 0u) {
                 const unsigned long long row = sTri[cube];
                 for (unsigned i = 0; i < nTri; ++i) {
                     const unsigned addr = sBase + off + i;
@@ -188,10 +198,26 @@ mc_extract_kernel(const __grid_constant__ McArgs a) {
             }
             __syncthreads();                                                                                           // the tile and the counters are reused
         }
+        if (kCount && tid == 0) a.chunkCounts[chunk] = sChunk;
     }
 }
 
 __global__ void mc_reset_kernel(unsigned* count) { *count = 0; }
+// the count pass's total: one CTA sums the chunk counts (integers: the same sum in any order)
+#define BF_MC_SUM_THREADS 256
+__global__ void __launch_bounds__(BF_MC_SUM_THREADS) mc_total_kernel(const unsigned* chunkCounts, unsigned numChunks, unsigned long long* total) {
+    __shared__ unsigned long long sSum[BF_MC_SUM_THREADS];
+    const unsigned tid = threadIdx.x;
+    unsigned long long s = 0;
+    for (unsigned c = tid; c < numChunks; c += BF_MC_SUM_THREADS) s += chunkCounts[c];
+    sSum[tid] = s;
+    __syncthreads();
+    for (unsigned w = BF_MC_SUM_THREADS / 2; w > 0; w >>= 1) {
+        if (tid < w) sSum[tid] += sSum[tid + w];
+        __syncthreads();
+    }
+    if (tid == 0) *total = sSum[0];
+}
 __global__ void mc_clamp_kernel(unsigned* count, unsigned maxNumTriangles, const BFMarchingCubesParams* d_params) {
     const unsigned cap = d_params ? d_params->m_maxNumTriangles : maxNumTriangles;
     if (*count > cap) *count = cap;                                                                                     // appendTriangle, MarchingCubesSDFUtil.h:252-263
@@ -206,16 +232,57 @@ static int check_args(const BFHashDataStruct* hd, const BFHashParams* hp, const 
     return 0;
 }
 
-static int do_extract(const BFHashDataStruct* hd, const BFHashParams* hp, const BFMarchingCubesParams* p, const BFMarchingCubesParams* d_params, BFMarchingCubesTriangle* tri, unsigned* count) {
+static unsigned num_chunks(const BFHashParams* hp) { return (unsigned)(((size_t)hp->m_hashNumBuckets * BF_HASH_BUCKET_SIZE + BF_MC_THREADS - 1) / BF_MC_THREADS); }
+
+// the one launch of either pass: a resident grid (at most two CTAs per SM) strides over chunks [a.chunkBegin, a.chunkEnd), which must not be empty
+template <bool kCount>
+static void launch_chunks(const McArgs& a) {
+    const unsigned grid = std::min<unsigned>(a.chunkEnd - a.chunkBegin, (unsigned)num_sms() * 2);
+    ++g_launchCount;
+    mc_extract_kernel<kCount><<<grid, BF_MC_THREADS, 0, stream()>>>(a);
+}
+
+static void launch_reset(unsigned* count) {
+    ++g_launchCount;
+    mc_reset_kernel<<<1, 1, 0, stream()>>>(count);
+}
+
+// extraction of the blocks in chunks [chunkBegin, chunkEnd), then the clamp; h_found (pinned, may be NULL) receives the count before the clamp
+static int do_extract(const BFHashDataStruct* hd, const BFHashParams* hp, const BFMarchingCubesParams* p, const BFMarchingCubesParams* d_params, BFMarchingCubesTriangle* tri, unsigned* count,
+                      unsigned chunkBegin, unsigned chunkEnd, unsigned* h_found) {
     const int bad = check_args(hd, hp, p, tri, count);
     if (bad) return bad;
     McArgs a;
     a.hd = *hd; a.hp = *hp; a.p = *p; a.d_params = d_params; a.tri = tri; a.count = count;
-    const size_t chunks = ((size_t)hp->m_hashNumBuckets * BF_HASH_BUCKET_SIZE + BF_MC_THREADS - 1) / BF_MC_THREADS;
-    const unsigned grid = (unsigned)std::min<size_t>(chunks, (size_t)num_sms() * 2);
-    g_launchCount += 2;
-    mc_extract_kernel<<<grid, BF_MC_THREADS, 0, stream()>>>(a);
+    a.chunkBegin = chunkBegin; a.chunkEnd = chunkEnd; a.chunkCounts = nullptr;
+    if (chunkEnd > chunkBegin) launch_chunks<false>(a);
+    if (h_found) BF_CHECK(cudaMemcpyAsync(h_found, count, sizeof(unsigned), cudaMemcpyDeviceToHost, stream()));
+    ++g_launchCount;
     mc_clamp_kernel<<<1, 1, 0, stream()>>>(count, p->m_maxNumTriangles, d_params);
+    BF_CHECK(cudaGetLastError());
+    return 0;
+}
+
+static int mc_refuse(const char* where, const char* why) {
+    set_last_error((std::string(where) + ": " + why).c_str(), cudaErrorInvalidValue);
+    return (int)cudaErrorInvalidValue;
+}
+// the refusals of the count and range entry points, before anything is enqueued
+static int check_range_args(const char* where, const BFHashDataStruct* hd, const BFHashParams* hp, const BFMarchingCubesParams* p, const void* out, const void* counter) {
+    if (!hd || !hp || !p || !out) return mc_refuse(where, "NULL argument");
+    if (!counter) return mc_refuse(where, "NULL counter");
+    if (check_args(hd, hp, p, reinterpret_cast<const BFMarchingCubesTriangle*>(out), reinterpret_cast<const unsigned*>(counter)))
+        return mc_refuse(where, "hash or cell parameters the kernel does not take (bucket count 0, voxel size, block or bucket size, bucket count of the parameters)");
+    return 0;
+}
+
+static int do_count(const BFHashDataStruct* hd, const BFHashParams* hp, const BFMarchingCubesParams* p, unsigned* chunkCounts, unsigned long long* total) {
+    McArgs a;
+    a.hd = *hd; a.hp = *hp; a.p = *p; a.d_params = nullptr; a.tri = nullptr; a.count = nullptr;
+    a.chunkBegin = 0; a.chunkEnd = num_chunks(hp); a.chunkCounts = chunkCounts;
+    launch_chunks<true>(a);
+    ++g_launchCount;
+    mc_total_kernel<<<1, BF_MC_SUM_THREADS, 0, stream()>>>(chunkCounts, a.chunkEnd, total);
     BF_CHECK(cudaGetLastError());
     return 0;
 }
@@ -322,25 +389,50 @@ struct BFMarchingCubes {
     unsigned* h_numTriangles = nullptr;                  // pinned
     std::vector<float> positions, colors;                // m_meshData: soup, three vertices per triangle
     std::vector<BFMarchingCubesTriangle> staging;
+    unsigned* d_chunkCounts = nullptr;                   // the whole-mesh call's count pass: triangles per chunk, device and pinned
+    unsigned* h_chunkCounts = nullptr;
+    unsigned chunkCapacity = 0;
+    unsigned long long* d_total = nullptr;
+    unsigned long long* h_total = nullptr;               // pinned
+    unsigned long long lastFound = 0, lastKept = 0;      // the last extraction: triangles its cells produced, triangles in the mesh buffer
 };
 
 BF_API void resetMarchingCubesCUDA(BFMarchingCubesData* data) {
     if (!data || !data->d_numTriangles) BF_SAFE((int)cudaErrorInvalidValue);
-    ++g_launchCount;
-    mc_reset_kernel<<<1, 1, 0, stream()>>>(data->d_numTriangles);
+    launch_reset(data->d_numTriangles);
     BF_SAFE((int)cudaGetLastError());
 }
 BF_API void extractIsoSurfaceCUDA(const BFHashDataStruct* hashData, const BFRayCastData*, const BFMarchingCubesParams* params, BFMarchingCubesData* data) {
     if (!data || !data->d_params) BF_SAFE((int)cudaErrorInvalidValue);
-    BF_SAFE(do_extract(hashData, bound_hash_params(), params, data->d_params, data->d_triangles, data->d_numTriangles));
+    const BFHashParams* hp = bound_hash_params();
+    BF_SAFE(do_extract(hashData, hp, params, data->d_params, data->d_triangles, data->d_numTriangles, 0, hp ? num_chunks(hp) : 0, nullptr));
+}
+// reset + extraction of chunks [chunkBegin, chunkEnd) (arguments already checked)
+static int extract_chunks(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params, BFMarchingCubesTriangle* d_triangles,
+                          uint32_t* d_numTriangles, unsigned chunkBegin, unsigned chunkEnd, unsigned* h_found) {
+    launch_reset(d_numTriangles);
+    return do_extract(hashData, hashParams, params, nullptr, d_triangles, d_numTriangles, chunkBegin, chunkEnd, h_found);
 }
 BF_API int bfMarchingCubesExtract(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params, BFMarchingCubesTriangle* d_triangles,
                                   uint32_t* d_numTriangles) {
     const int bad = check_args(hashData, hashParams, params, d_triangles, d_numTriangles);
     if (bad) return bad;
-    ++g_launchCount;
-    mc_reset_kernel<<<1, 1, 0, stream()>>>(d_numTriangles);
-    return do_extract(hashData, hashParams, params, nullptr, d_triangles, d_numTriangles);
+    return extract_chunks(hashData, hashParams, params, d_triangles, d_numTriangles, 0, num_chunks(hashParams), nullptr);
+}
+BF_API int bfMarchingCubesCount(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params, uint32_t* d_chunkCounts,
+                                unsigned long long* d_total) {
+    const int bad = check_range_args("bfMarchingCubesCount", hashData, hashParams, params, d_chunkCounts, d_total);
+    if (bad) return bad;
+    return do_count(hashData, hashParams, params, d_chunkCounts, d_total);
+}
+BF_API int bfMarchingCubesExtractRange(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params, uint32_t chunkBegin, uint32_t chunkEnd,
+                                       BFMarchingCubesTriangle* d_triangles, uint32_t* d_numTriangles) {
+    const char* where = "bfMarchingCubesExtractRange";
+    const int bad = check_range_args(where, hashData, hashParams, params, d_triangles, d_numTriangles);
+    if (bad) return bad;
+    if (chunkBegin > chunkEnd) return mc_refuse(where, "chunkBegin > chunkEnd");
+    if (chunkEnd > num_chunks(hashParams)) return mc_refuse(where, "chunk range past the table");
+    return extract_chunks(hashData, hashParams, params, d_triangles, d_numTriangles, chunkBegin, chunkEnd, nullptr);
 }
 
 BF_API int bfMarchingCubesCreate(const BFMarchingCubesParams* params, BFMarchingCubes** out) {
@@ -349,7 +441,7 @@ BF_API int bfMarchingCubesCreate(const BFMarchingCubesParams* params, BFMarching
     mc->params = *params;
     cudaError_t e = cudaMalloc(&mc->d_triangles, sizeof(BFMarchingCubesTriangle) * (size_t)params->m_maxNumTriangles);
     if (e == cudaSuccess) e = cudaMalloc(&mc->d_numTriangles, sizeof(unsigned));
-    if (e == cudaSuccess) e = cudaMallocHost(&mc->h_numTriangles, sizeof(unsigned));
+    if (e == cudaSuccess) e = cudaMallocHost(&mc->h_numTriangles, 2 * sizeof(unsigned));             // the count after and before the clamp
     if (e != cudaSuccess) { bfMarchingCubesDestroy(mc); set_last_error("bfMarchingCubesCreate", e); return (int)e; }
     *out = mc;
     return 0;
@@ -357,23 +449,12 @@ BF_API int bfMarchingCubesCreate(const BFMarchingCubesParams* params, BFMarching
 BF_API void bfMarchingCubesDestroy(BFMarchingCubes* mc) {
     if (!mc) return;
     cudaFree(mc->d_triangles); cudaFree(mc->d_numTriangles); cudaFreeHost(mc->h_numTriangles);
+    cudaFree(mc->d_chunkCounts); cudaFreeHost(mc->h_chunkCounts); cudaFree(mc->d_total); cudaFreeHost(mc->h_total);
     delete mc;
 }
-BF_API int bfMarchingCubesExtractIsoSurface(BFMarchingCubes* mc, const BFHashDataStruct* hashData, const BFHashParams* hashParams, const float* minCorner, const float* maxCorner,
-                                            int boxEnabled) {
-    if (!mc) return (int)cudaErrorInvalidValue;
-    for (int k = 0; k < 3; ++k) { mc->params.m_minCorner[k] = minCorner ? minCorner[k] : 0.0f; mc->params.m_maxCorner[k] = maxCorner ? maxCorner[k] : 0.0f; }
-    mc->params.m_boxEnabled = boxEnabled ? 1 : 0;
-    const int rc = bfMarchingCubesExtract(hashData, hashParams, &mc->params, mc->d_triangles, mc->d_numTriangles);
-    if (rc) return rc;
-    // copyTrianglesToCPU: the count first, then only the triangles there are (the reference copies the whole buffer)
-    BF_CHECK(cudaMemcpyAsync(mc->h_numTriangles, mc->d_numTriangles, sizeof(unsigned), cudaMemcpyDeviceToHost, stream()));
-    BF_CHECK(cudaStreamSynchronize(stream()));
-    const unsigned n = *mc->h_numTriangles;
-    if (n == 0) return 0;
-    mc->staging.resize(n);
-    BF_CHECK(cudaMemcpyAsync(mc->staging.data(), mc->d_triangles, sizeof(BFMarchingCubesTriangle) * (size_t)n, cudaMemcpyDeviceToHost, stream()));
-    BF_CHECK(cudaStreamSynchronize(stream()));
+
+// copyTrianglesToCPU's append: n triangles from the staging buffer to the end of the host mesh buffer
+static void append_staged(BFMarchingCubes* mc, unsigned n) {
     const size_t base = mc->positions.size() / 3;
     mc->positions.resize((base + 3 * (size_t)n) * 3); mc->colors.resize((base + 3 * (size_t)n) * 4);
     const BFMarchingCubesVertex* v = reinterpret_cast<const BFMarchingCubesVertex*>(mc->staging.data());
@@ -382,6 +463,111 @@ BF_API int bfMarchingCubesExtractIsoSurface(BFMarchingCubes* mc, const BFHashDat
         p[0] = v[i].p[0]; p[1] = v[i].p[1]; p[2] = v[i].p[2];
         c[0] = v[i].c[0]; c[1] = v[i].c[1]; c[2] = v[i].c[2]; c[3] = 1.0f;                   // vec4f(vec3f): w = 1
     }
+}
+static void set_box(BFMarchingCubes* mc, const float* minCorner, const float* maxCorner, int boxEnabled) {
+    for (int k = 0; k < 3; ++k) { mc->params.m_minCorner[k] = minCorner ? minCorner[k] : 0.0f; mc->params.m_maxCorner[k] = maxCorner ? maxCorner[k] : 0.0f; }
+    mc->params.m_boxEnabled = boxEnabled ? 1 : 0;
+}
+
+BF_API int bfMarchingCubesExtractIsoSurface(BFMarchingCubes* mc, const BFHashDataStruct* hashData, const BFHashParams* hashParams, const float* minCorner, const float* maxCorner,
+                                            int boxEnabled) {
+    if (!mc) return (int)cudaErrorInvalidValue;
+    set_box(mc, minCorner, maxCorner, boxEnabled);
+    const int bad = check_args(hashData, hashParams, &mc->params, mc->d_triangles, mc->d_numTriangles);
+    if (bad) return bad;
+    // the count before the clamp goes to h_numTriangles[1], so that a full buffer's loss is on record
+    const int rc = extract_chunks(hashData, hashParams, &mc->params, mc->d_triangles, mc->d_numTriangles, 0, num_chunks(hashParams), mc->h_numTriangles + 1);
+    if (rc) return rc;
+    // copyTrianglesToCPU: the count first, then only the triangles there are (the reference copies the whole buffer)
+    BF_CHECK(cudaMemcpyAsync(mc->h_numTriangles, mc->d_numTriangles, sizeof(unsigned), cudaMemcpyDeviceToHost, stream()));
+    BF_CHECK(cudaStreamSynchronize(stream()));
+    const unsigned n = *mc->h_numTriangles;
+    mc->lastFound = mc->h_numTriangles[1]; mc->lastKept = n;
+    if (n == 0) return 0;
+    mc->staging.resize(n);
+    BF_CHECK(cudaMemcpyAsync(mc->staging.data(), mc->d_triangles, sizeof(BFMarchingCubesTriangle) * (size_t)n, cudaMemcpyDeviceToHost, stream()));
+    BF_CHECK(cudaStreamSynchronize(stream()));
+    append_staged(mc, n);
+    return 0;
+}
+
+BF_API int bfMarchingCubesExtractIsoSurfaceWhole(BFMarchingCubes* mc, const BFHashDataStruct* hashData, const BFHashParams* hashParams, const float* minCorner,
+                                                 const float* maxCorner, int boxEnabled, BFMarchingCubesWholeInfo* info) {
+    const char* where = "bfMarchingCubesExtractIsoSurfaceWhole";
+    if (!mc || !info) return mc_refuse(where, "NULL argument");
+    set_box(mc, minCorner, maxCorner, boxEnabled);
+    if (check_args(hashData, hashParams, &mc->params, mc->d_triangles, mc->d_numTriangles))
+        return mc_refuse(where, "hash or cell parameters the kernel does not take (bucket count 0, voxel size, block or bucket size, bucket count of the parameters)");
+    BFMarchingCubesWholeInfo r;
+    memset(&r, 0, sizeof(r));
+    // 1. the count pass, and its chunk counts and total read back: the first host synchronisation
+    const unsigned chunks = num_chunks(hashParams);
+    if (chunks > mc->chunkCapacity) {
+        cudaFree(mc->d_chunkCounts); cudaFreeHost(mc->h_chunkCounts);
+        mc->d_chunkCounts = nullptr; mc->h_chunkCounts = nullptr; mc->chunkCapacity = 0;
+        cudaError_t e = cudaMalloc(&mc->d_chunkCounts, sizeof(unsigned) * (size_t)chunks);
+        if (e == cudaSuccess) e = cudaMallocHost(&mc->h_chunkCounts, sizeof(unsigned) * (size_t)chunks);
+        if (e != cudaSuccess) { set_last_error(where, e); return (int)e; }
+        mc->chunkCapacity = chunks;
+    }
+    if (!mc->d_total) {
+        cudaError_t e = cudaMalloc(&mc->d_total, sizeof(unsigned long long));
+        if (e == cudaSuccess) e = cudaMallocHost(&mc->h_total, sizeof(unsigned long long));
+        if (e != cudaSuccess) { set_last_error(where, e); return (int)e; }
+    }
+    int rc = do_count(hashData, hashParams, &mc->params, mc->d_chunkCounts, mc->d_total);
+    if (rc) return rc;
+    BF_CHECK(cudaMemcpyAsync(mc->h_chunkCounts, mc->d_chunkCounts, sizeof(unsigned) * (size_t)chunks, cudaMemcpyDeviceToHost, stream()));
+    BF_CHECK(cudaMemcpyAsync(mc->h_total, mc->d_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream()));
+    BF_CHECK(cudaStreamSynchronize(stream()));
+    r.chunks = chunks;
+    r.trianglesCounted = *mc->h_total;
+    r.hostSyncs = 1;
+    // 2. the buffer rule: the parts are cut between chunks, so a chunk that holds more triangles than the buffer enlarges it to that chunk
+    unsigned largestChunk = 0;
+    for (unsigned c = 0; c < chunks; ++c) largestChunk = std::max(largestChunk, mc->h_chunkCounts[c]);
+    if (largestChunk > mc->params.m_maxNumTriangles) {
+        BFMarchingCubesTriangle* t = nullptr;
+        const cudaError_t e = cudaMalloc(&t, sizeof(BFMarchingCubesTriangle) * (size_t)largestChunk);
+        if (e != cudaSuccess) { set_last_error("bfMarchingCubesExtractIsoSurfaceWhole: enlarging the triangle buffer", e); return (int)e; }      // the old buffer stays
+        cudaFree(mc->d_triangles);
+        mc->d_triangles = t;
+        mc->params.m_maxNumTriangles = largestChunk;
+        r.bufferEnlarged = 1;
+    }
+    r.bufferTriangles = mc->params.m_maxNumTriangles;
+    // 3. consecutive chunks, greedily, into parts of at most m_maxNumTriangles; each part extracted, copied back and appended, one synchronisation each
+    const unsigned cap = mc->params.m_maxNumTriangles;
+    unsigned begin = 0;
+    unsigned long long sum = 0;
+    for (unsigned c = 0; c <= chunks; ++c) {
+        if (c < chunks && sum + mc->h_chunkCounts[c] <= cap) { sum += mc->h_chunkCounts[c]; continue; }
+        if (sum != 0) {                                                                  // chunks [begin, c): an empty part is not extracted
+            const unsigned want = (unsigned)sum;
+            rc = extract_chunks(hashData, hashParams, &mc->params, mc->d_triangles, mc->d_numTriangles, begin, c, nullptr);
+            if (rc) return rc;
+            BF_CHECK(cudaMemcpyAsync(mc->h_numTriangles, mc->d_numTriangles, sizeof(unsigned), cudaMemcpyDeviceToHost, stream()));
+            mc->staging.resize(want);
+            BF_CHECK(cudaMemcpyAsync(mc->staging.data(), mc->d_triangles, sizeof(BFMarchingCubesTriangle) * (size_t)want, cudaMemcpyDeviceToHost, stream()));
+            BF_CHECK(cudaStreamSynchronize(stream()));
+            const unsigned got = *mc->h_numTriangles;
+            append_staged(mc, std::min(got, want));
+            r.trianglesExtracted += got;
+            r.parts += 1;
+            r.largestPart = std::max(r.largestPart, got);
+            r.hostSyncs += 1;
+        }
+        begin = c;
+        sum = c < chunks ? mc->h_chunkCounts[c] : 0;
+    }
+    mc->lastFound = r.trianglesCounted; mc->lastKept = r.trianglesExtracted;
+    *info = r;
+    return 0;
+}
+
+BF_API int bfMarchingCubesGetLastExtraction(const BFMarchingCubes* mc, unsigned long long* found, unsigned long long* kept) {
+    if (!mc || !found || !kept) return (int)cudaErrorInvalidValue;
+    *found = mc->lastFound; *kept = mc->lastKept;
     return 0;
 }
 BF_API void bfMarchingCubesClearMeshBuffer(BFMarchingCubes* mc) { if (mc) { mc->positions.clear(); mc->colors.clear(); } }

@@ -233,20 +233,29 @@ def fit_hash_params(base_hp, voxel_size: float, counter, max_table_bytes: int | 
     return hp, report
 
 
-def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6_000_000) -> dict:
-    """iso-surface of a scene (threshold 10 x voxel, the reference's s_SDFMarchingCubeThreshFactor) saved as PLY"""
+def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6_000_000, whole: bool = False) -> dict:
+    """iso-surface of a scene (threshold 10 x voxel, the reference's s_SDFMarchingCubeThreshFactor) saved as PLY.  Returns {"triangles" (in the
+    mesh), "triangles_found" (the cells produced), "triangles_dropped" (found - kept: what a full buffer of max_num_triangles lost), "mesh_path"}.
+    whole=True extracts through CUDAMarchingCubesHashSDF.extractIsoSurfaceWhole -- counted first, then in parts that fit the buffer, so nothing
+    is dropped -- and adds its report under "mesh"."""
     hp = scene.m_hashParams
     mc = CUDAMarchingCubesHashSDF(marching_cubes_params(int(hp.m_hashNumBuckets), float(hp.m_virtualVoxelSize), max_num_triangles), device)
     try:
-        tri = mc.extractIsoSurface(scene) // 3
-        return {"triangles": tri, "mesh_path": mc.saveMesh(ply_path, overwrite=True)}
+        out = {}
+        if whole:
+            out["mesh"] = mc.extractIsoSurfaceWhole(scene)
+        else:
+            mc.extractIsoSurface(scene)
+        found, kept = mc.lastExtraction()
+        out.update(triangles=kept, triangles_found=found, triangles_dropped=found - kept, mesh_path=mc.saveMesh(ply_path, overwrite=True))
+        return out
     finally:
         mc.close()
 
 
 def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: float = 0.004, poses="recorded", hash_buckets: int | None = None,
                    sdf_blocks: int | None = None, device="cuda:0", max_frames: int | None = None, scene: CUDASceneRepHashSDF | None = None,
-                   max_num_triangles: int = 6_000_000, fit_hash: bool = False, max_table_bytes: int | None = None) -> dict:
+                   max_num_triangles: int = 6_000_000, fit_hash: bool = False, max_table_bytes: int | None = None, whole_mesh: bool = False) -> dict:
     """Fuses a .sens recording along fixed camera-to-world poses -- "recorded" (the poses stored with the frames) or an array [n, 4, 4] --
     into a voxel hash of voxel_size (or into ``scene``, a reset CUDASceneRepHashSDF), with no bundling.  Frames whose pose is not finite are
     skipped.  Returns {"frames", "fused", "skipped", "batches", "inserts_dropped" (block inserts the hash had no room for), "heap_free",
@@ -254,7 +263,9 @@ def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: floa
     fit_hash=True sizes the hash from the blocks the fusion will allocate: a first pass decodes and ingests every frame as the fusion does and
     counts them (BlockCounter), fit_hash_params sizes the hash (within max_table_bytes), and the fusion runs as a second pass.  The result then
     also holds "blocks_counted", "buckets", "predicted_overflow" (0 unless max_table_bytes was too small to avoid overflow) and the whole
-    report under "fit".  fit_hash excludes hash_buckets, sdf_blocks and scene."""
+    report under "fit".  fit_hash excludes hash_buckets, sdf_blocks and scene.
+    The mesh: "triangles_found" and "triangles_dropped" as mesh_scene reports them; whole_mesh=True meshes through mesh_scene(whole=True), which
+    drops nothing however small max_num_triangles is, and adds its report under "mesh"."""
     import torch
     if fit_hash and (hash_buckets is not None or sdf_blocks is not None or scene is not None):
         raise ValueError("fit_hash sizes the hash itself: pass no hash_buckets, sdf_blocks or scene")
@@ -313,9 +324,9 @@ def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: floa
         out["heap_free"] = scene.getHeapFreeCount()
         if fit is not None:
             out.update(blocks_counted=fit["blocks_counted"], buckets=fit["buckets"], predicted_overflow=fit["predicted_overflow"], fit=fit)
-        out.update(triangles=0, mesh_path=None, scene=scene)
+        out.update(triangles=0, triangles_found=0, triangles_dropped=0, mesh_path=None, scene=scene)
         if ply_path is not None:
-            out.update(mesh_scene(scene, ply_path, device, max_num_triangles))
+            out.update(mesh_scene(scene, ply_path, device, max_num_triangles, whole=whole_mesh))
         return out
     finally:
         r.close()

@@ -33,8 +33,17 @@ def _bind(L):
     L.bfMeshMergeCloseVertices.argtypes = [vp, vp, sz, vp, sz, C.c_float, C.POINTER(sz), C.POINTER(sz)]
     L.bfMeshRemoveDuplicateFaces.argtypes = [vp, sz, C.POINTER(sz)]
     L.bfMeshSavePly.argtypes = [C.c_char_p, vp, vp, sz, vp, sz]
+    L.bfMarchingCubesCount.argtypes = [vp, vp, vp, vp, vp]
+    L.bfMarchingCubesExtractRange.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp]
+    L.bfMarchingCubesExtractIsoSurfaceWhole.argtypes = [vp, vp, vp, vp, vp, C.c_int, vp]
+    L.bfMarchingCubesGetLastExtraction.argtypes = [vp, C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
     L._mc_bound = True
     return L
+
+
+def num_chunks(num_buckets: int) -> int:
+    """chunks of a table of num_buckets buckets: the count pass writes one triangle count per chunk"""
+    return (int(num_buckets) * capi.BF_HASH_BUCKET_SIZE + capi.BF_MC_CHUNK_SLOTS - 1) // capi.BF_MC_CHUNK_SLOTS
 
 
 def merge_close_vertices(positions: np.ndarray, colors: np.ndarray | None, faces: np.ndarray, thresh: float = 0.00001):
@@ -90,6 +99,44 @@ class CUDAMarchingCubesHashSDF:
         lo = (C.c_float * 3)(*min_corner); hi = (C.c_float * 3)(*max_corner)
         capi.check(self.lib.bfMarchingCubesExtractIsoSurface(self._h, C.byref(scene.m_hashData), C.byref(scene.m_hashParams), lo, hi, 1 if box_enabled else 0), "bfMarchingCubesExtractIsoSurface")
         return int(self.lib.bfMarchingCubesGetSoup(self._h, None, None))
+
+    def _box_params(self, scene, min_corner, max_corner, box_enabled):
+        p = BFMarchingCubesParams()
+        C.memmove(C.byref(p), C.byref(self.m_params), C.sizeof(BFMarchingCubesParams))
+        p.m_boxEnabled = 1 if box_enabled else 0
+        for k in range(3):
+            p.m_minCorner[k], p.m_maxCorner[k] = min_corner[k], max_corner[k]
+        p.m_hashNumBuckets = int(scene.m_hashParams.m_hashNumBuckets)
+        return p
+
+    def count(self, scene, min_corner=(0.0, 0.0, 0.0), max_corner=(0.0, 0.0, 0.0), box_enabled: bool = False):
+        """the count pass (bfMarchingCubesCount) -> (total triangles, triangles per 512-slot chunk of the table: uint32 numpy array).  Synchronises once."""
+        t = self._torch
+        self._bind_stream()
+        p = self._box_params(scene, min_corner, max_corner, box_enabled)
+        counts = t.empty(num_chunks(p.m_hashNumBuckets), dtype=t.int32, device=self.device)
+        total = t.empty(1, dtype=t.int64, device=self.device)
+        capi.check(self.lib.bfMarchingCubesCount(C.byref(scene.m_hashData), C.byref(scene.m_hashParams), C.byref(p), counts.data_ptr(), total.data_ptr()),
+                   "bfMarchingCubesCount")
+        return int(total.item()), counts.cpu().numpy().view(np.uint32)
+
+    def extractIsoSurfaceWhole(self, scene, min_corner=(0.0, 0.0, 0.0), max_corner=(0.0, 0.0, 0.0), box_enabled: bool = False) -> dict:
+        """the whole mesh appended to the mesh buffer, in parts that fit the buffer (bfMarchingCubesExtractIsoSurfaceWhole): no triangle is dropped.
+        Returns {"triangles_counted", "triangles_extracted", "chunks", "parts", "largest_part", "buffer_triangles", "buffer_enlarged", "host_syncs"}."""
+        self._bind_stream()
+        lo = (C.c_float * 3)(*min_corner); hi = (C.c_float * 3)(*max_corner)
+        info = capi.BFMarchingCubesWholeInfo()
+        capi.check(self.lib.bfMarchingCubesExtractIsoSurfaceWhole(self._h, C.byref(scene.m_hashData), C.byref(scene.m_hashParams), lo, hi, 1 if box_enabled else 0,
+                                                                  C.byref(info)), "bfMarchingCubesExtractIsoSurfaceWhole")
+        return {"triangles_counted": int(info.trianglesCounted), "triangles_extracted": int(info.trianglesExtracted), "chunks": int(info.chunks),
+                "parts": int(info.parts), "largest_part": int(info.largestPart), "buffer_triangles": int(info.bufferTriangles),
+                "buffer_enlarged": bool(info.bufferEnlarged), "host_syncs": int(info.hostSyncs)}
+
+    def lastExtraction(self) -> tuple[int, int]:
+        """(found, kept) of the last extraction: triangles its cells produced and triangles it appended; found > kept when a full buffer dropped some"""
+        found, kept = C.c_ulonglong(0), C.c_ulonglong(0)
+        capi.check(self.lib.bfMarchingCubesGetLastExtraction(self._h, C.byref(found), C.byref(kept)), "bfMarchingCubesGetLastExtraction")
+        return int(found.value), int(kept.value)
 
     def soup(self):
         """the mesh buffer: (positions [n, 3], colours [n, 4]) float32 copies, three consecutive vertices per triangle"""

@@ -9,6 +9,10 @@ the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every 
         [--fit-hash]                size that fused hash from a count of the blocks it will hold (fuse.fit_hash_params), so it drops nothing
         [--grow-hash MAX_BLOCKS]    start the online hash at --sdf-blocks and let the loop grow it up to MAX_BLOCKS voxel blocks while it scans
         [--device-frames N]         keep N frame slots on the device and every frame in pinned host memory (same results, less device memory)
+        [--whole-mesh]              count the mesh's triangles first and extract them in parts that fit the triangle buffer, so none is dropped
+
+The JSON summary always carries "triangles_found" (what the iso-surface's cells produced) and "triangles_dropped" (what a full triangle buffer
+lost: found - kept); with --whole-mesh it is 0, and the extraction's report (parts, buffer, synchronisations) goes under "mesh".
 """
 from __future__ import annotations
 
@@ -21,7 +25,6 @@ import numpy as np
 from . import _capi as capi
 from . import fuse
 from .frame_loop import FrameLoop, default_params
-from .marching_cubes import CUDAMarchingCubesHashSDF, marching_cubes_params
 from .scene_rep import CUDASceneRepHashSDF
 from .sens import SensorDataReader
 
@@ -37,7 +40,7 @@ class _LoopScene:
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
                 sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None,
                 mesh_voxel_size: float | None = None, fit_hash: bool = False, grow_hash: int | None = None,
-                device_frames: int | None = None) -> dict:
+                device_frames: int | None = None, whole_mesh: bool = False) -> dict:
     """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
     solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
     global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
@@ -46,7 +49,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
     fit_hash that hash is sized by FrameLoop.fit_hash_params, whose report goes under "fit".  grow_hash=MAX_BLOCKS: the online hash starts at
     sdf_blocks (default: the loop's) and the loop may grow it up to MAX_BLOCKS voxel blocks (hashMaxSDFBlocks); FrameLoop.hash_growth() goes
     under "hash".  device_frames=N keeps N frame slots on the device over a pinned host store of every frame (deviceFrameSlots); the results
-    do not change, and FrameLoop.frame_store() goes under "frame_store"."""
+    do not change, and FrameLoop.frame_store() goes under "frame_store".  The mesh adds "triangles_found" and "triangles_dropped"
+    (fuse.mesh_scene); whole_mesh=True extracts it counted and in parts that fit the buffer, dropping nothing, and adds the report under "mesh"."""
     r = SensorDataReader(sens_path)
     n = len(r) if max_frames is None else min(len(r), max_frames)
     P = fuse.recording_params(r.header, n)
@@ -78,7 +82,7 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
             loop.step_past_end()
     loop.join()
     out = {"frames": n, "valid": int(sum(s["validTransform"] for s in status)), "keyframes": loop.counters()["keyframes"], "trajectory": loop.trajectory(n), "status": status,
-           "mesh_path": None, "triangles": 0}
+           "mesh_path": None, "triangles": 0, "triangles_found": 0, "triangles_dropped": 0}
     if finish is not None:
         out["finish"] = finish
     if grow_hash is not None:
@@ -91,15 +95,11 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
         scene = CUDASceneRepHashSDF(hp, device)
         out["fuse"] = loop.fuse(scene, n=n)
         if ply_path is not None:
-            out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles))
+            out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles, whole=whole_mesh))
         scene.close()
     elif ply_path is not None:
-        scene = _LoopScene(loop)                       # the table the loop holds now: a grown one has more buckets than P.hash
-        mp = marching_cubes_params(int(scene.m_hashParams.m_hashNumBuckets), float(scene.m_hashParams.m_virtualVoxelSize), max_num_triangles)
-        mc = CUDAMarchingCubesHashSDF(mp, device)
-        out["triangles"] = mc.extractIsoSurface(scene) // 3
-        out["mesh_path"] = mc.saveMesh(ply_path, overwrite=True)
-        mc.close()
+        # the table the loop holds now: a grown one has more buckets than P.hash
+        out.update(fuse.mesh_scene(_LoopScene(loop), ply_path, device, max_num_triangles, whole=whole_mesh))
     if device_frames is not None:
         out["frame_store"] = loop.frame_store()
     loop.close(); r.close()
@@ -155,6 +155,9 @@ def main(argv=None) -> int:
     ap.add_argument("--device-frames", type=int, default=None, metavar="N",
                     help="keep N frame slots on the device over a pinned host store of every frame, N >= 16 (the results do not change; the JSON "
                          "summary carries slots, bytes, fetches and hits under 'frame_store')")
+    ap.add_argument("--whole-mesh", action="store_true",
+                    help="count the iso-surface's triangles on the device and extract them in parts that fit the triangle buffer, so that none is "
+                         "dropped (the JSON summary carries the extraction's report under 'mesh')")
     a = ap.parse_args(argv)
     if a.fit_hash and a.poses != "recorded" and a.mesh_voxel_size is None:
         ap.error("--fit-hash sizes a fused hash: use it with --mesh-voxel-size or --poses recorded")
@@ -162,20 +165,26 @@ def main(argv=None) -> int:
         if a.fit_hash and (a.hash_buckets is not None or a.sdf_blocks is not None):
             ap.error("--fit-hash sizes the fused hash itself: drop --hash-buckets / --sdf-blocks")
         voxel = a.mesh_voxel_size if a.mesh_voxel_size is not None else float(default_params(16, 16).hash.m_virtualVoxelSize)
-        o = fuse.fuse_recording(a.sens, a.ply, voxel, "recorded", a.hash_buckets, a.sdf_blocks, a.device, a.frames, fit_hash=a.fit_hash)
+        o = fuse.fuse_recording(a.sens, a.ply, voxel, "recorded", a.hash_buckets, a.sdf_blocks, a.device, a.frames, fit_hash=a.fit_hash,
+                                whole_mesh=a.whole_mesh)
         o["scene"].close()
         summary = {"frames": o["frames"], "fuse": {k: o[k] for k in ("fused", "skipped", "batches", "inserts_dropped", "heap_free")},
-                   "triangles": o["triangles"], "mesh_path": o["mesh_path"]}
+                   "triangles": o["triangles"], "mesh_path": o["mesh_path"], "triangles_found": o["triangles_found"],
+                   "triangles_dropped": o["triangles_dropped"]}
         if "fit" in o:
             summary["fit"] = o["fit"]
+        if "mesh" in o:
+            summary["mesh"] = o["mesh"]
         print(json.dumps(summary))
         return 0
     o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit,
                     mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash, grow_hash=a.grow_hash,
-                    device_frames=a.device_frames)
+                    device_frames=a.device_frames, whole_mesh=a.whole_mesh)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
-    summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path")}
+    summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path", "triangles_found", "triangles_dropped")}
+    if "mesh" in o:
+        summary["mesh"] = o["mesh"]
     if "finish" in o:
         summary["finish"] = o["finish"]                     # its "valid": StopScanningAndExit's verdict on the reconstruction
     if "fuse" in o:

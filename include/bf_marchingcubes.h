@@ -14,6 +14,11 @@
  *
  * The reference appends triangles with one atomicAdd each, so the ORDER of its triangle soup differs from run to run; the parity statement is on the
  * multiset of triangles (each with its three vertices in the reference's order).  Here a block's triangles are contiguous and ordered by voxel.
+ *
+ * A fixed triangle buffer drops what does not fit, as the reference's appendTriangle does.  For a model of any size: bfMarchingCubesCount counts
+ * the triangles of every 512-slot chunk of the table on the device, bfMarchingCubesExtractRange extracts the blocks of a chunk range, and
+ * bfMarchingCubesExtractIsoSurfaceWhole meshes the whole model through the class's buffer in parts cut between chunks.  The class's fixed path
+ * keeps the count from before the clamp (bfMarchingCubesGetLastExtraction), so a loss is on record.
  */
 #ifndef BF_MARCHINGCUBES_H
 #define BF_MARCHINGCUBES_H
@@ -61,9 +66,27 @@ void resetMarchingCubesCUDA(BFMarchingCubesData* data);
 void extractIsoSurfaceCUDA(const BFHashDataStruct* hashData, const BFRayCastData* rayCastData, const BFMarchingCubesParams* params, BFMarchingCubesData* data);
 
 /* ---- bf* extension: explicit parameters, cudaError_t return codes, no host synchronisation ---- */
-/* reset + extraction in one call: *d_numTriangles = min(triangles found, params->m_maxNumTriangles) when the stream reaches the end of the call */
+/* reset + extraction in one call: *d_numTriangles = min(triangles found, params->m_maxNumTriangles) when the stream reaches the end of the call.
+ * Triangles past the capacity are dropped, and which ones survive depends on the order in which blocks reserve their ranges. */
 int bfMarchingCubesExtract(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params,
                            BFMarchingCubesTriangle* d_triangles, uint32_t* d_numTriangles);
+
+/* ---- meshing a model of any size in parts ----
+ * The table's slots are cut into chunks of BF_MC_CHUNK_SLOTS consecutive slots, ceil(4 * buckets / 512) of them; a chunk is what one CTA of the
+ * extraction processes.  Every triangle comes from the cells of exactly one block, and every block from one slot, so chunk ranges that
+ * partition the table partition the triangle multiset.  Neither call synchronises with the host; malformed calls return cudaErrorInvalidValue,
+ * enqueue nothing and name the reason in bfGetLastErrorString. */
+#define BF_MC_CHUNK_SLOTS 512
+/* the count pass: the extraction's cell tests (and params' box), no triangle written and no global atomic.  d_chunkCounts[c] (device, one entry
+ * per chunk) = triangles of the blocks in chunk c, written with a plain store by the one CTA that owns the chunk, so deterministic;
+ * *d_total = their sum.  params->m_maxNumTriangles is not read. */
+int bfMarchingCubesCount(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params, uint32_t* d_chunkCounts,
+                         unsigned long long* d_total);
+/* reset + extraction of the blocks whose slots lie in chunks [chunkBegin, chunkEnd); neighbour blocks outside the range are still read for the
+ * cells' samples.  *d_numTriangles as bfMarchingCubesExtract, whose launch the full range [0, chunks) is.  An empty range leaves *d_numTriangles = 0.
+ * Refused: chunkEnd past the table, chunkBegin > chunkEnd, a NULL counter. */
+int bfMarchingCubesExtractRange(const BFHashDataStruct* hashData, const BFHashParams* hashParams, const BFMarchingCubesParams* params, uint32_t chunkBegin,
+                                uint32_t chunkEnd, BFMarchingCubesTriangle* d_triangles, uint32_t* d_numTriangles);
 
 /* ---- host side: class CUDAMarchingCubesHashSDF ---- */
 typedef struct BFMarchingCubes BFMarchingCubes;
@@ -72,6 +95,28 @@ void bfMarchingCubesDestroy(BFMarchingCubes* mc);
 /* extractIsoSurface(hashData, hashParams, rayCastData, minCorner, maxCorner, boxEnabled) + copyTrianglesToCPU: the triangles are APPENDED to the host mesh buffer */
 int  bfMarchingCubesExtractIsoSurface(BFMarchingCubes* mc, const BFHashDataStruct* hashData, const BFHashParams* hashParams, const float* minCorner, const float* maxCorner,
                                       int boxEnabled);
+/* the whole mesh through the class's buffer, in as many parts as it takes (two or more host synchronisations):
+ *   1. bfMarchingCubesCount, then the chunk counts read back (one synchronisation);
+ *   2. if one chunk holds more triangles than the buffer (m_maxNumTriangles), the buffer is enlarged to that chunk's count and stays so;
+ *   3. consecutive chunks are cut greedily into parts of at most m_maxNumTriangles triangles; each non-empty part is extracted
+ *      (bfMarchingCubesExtractRange), copied back and appended to the host mesh buffer as bfMarchingCubesExtractIsoSurface appends (one
+ *      synchronisation per part).
+ * saveMesh then applies unchanged.  No triangle is dropped: trianglesExtracted == trianglesCounted. */
+typedef struct BFMarchingCubesWholeInfo {
+    uint64_t trianglesCounted;              /* the count pass's total */
+    uint64_t trianglesExtracted;            /* the triangles the parts' extractions produced (appended to the mesh buffer) */
+    uint32_t chunks;                        /* chunks of the table */
+    uint32_t parts;                         /* non-empty parts extracted */
+    uint32_t largestPart;                   /* triangles of the largest part */
+    uint32_t bufferTriangles;               /* the buffer's capacity after the call */
+    uint32_t bufferEnlarged;                /* 1: a chunk held more triangles than the buffer had room for */
+    uint32_t hostSyncs;                     /* host synchronisations: 1 + parts */
+} BFMarchingCubesWholeInfo;
+int  bfMarchingCubesExtractIsoSurfaceWhole(BFMarchingCubes* mc, const BFHashDataStruct* hashData, const BFHashParams* hashParams, const float* minCorner,
+                                           const float* maxCorner, int boxEnabled, BFMarchingCubesWholeInfo* info);
+/* the last extraction of either call: *found = triangles its cells produced, *kept = triangles it appended to the mesh buffer.  found > kept
+ * means a full buffer dropped found - kept triangles (bfMarchingCubesExtractIsoSurface; the whole-mesh call drops none). */
+int  bfMarchingCubesGetLastExtraction(const BFMarchingCubes* mc, unsigned long long* found, unsigned long long* kept);
 void bfMarchingCubesClearMeshBuffer(BFMarchingCubes* mc);
 /* the host mesh buffer: triangle soup, three vertices per triangle; pointers stay valid until the next call on `mc` */
 size_t bfMarchingCubesGetSoup(const BFMarchingCubes* mc, const float** positions /* [n][3] */, const float** colors /* [n][4], alpha 1 */);
