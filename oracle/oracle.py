@@ -149,6 +149,14 @@ def canonical_blocks(snap: dict):
     return ent[:, :3].copy(), snap["voxels"][slots]
 
 
+def block_hash(pos, num_buckets: int | None = None) -> np.ndarray:
+    """VoxelUtilHashSDF.h:226-234 on (N, 3) block positions in uint32 arithmetic: (x*73856093) ^ (y*19349669) ^ (z*83492791), and with
+    num_buckets its bucket (an unsigned modulo)"""
+    p = np.asarray(pos, np.int64).reshape(-1, 3).astype(np.uint32)
+    v = (p[:, 0] * np.uint32(73856093)) ^ (p[:, 1] * np.uint32(19349669)) ^ (p[:, 2] * np.uint32(83492791))
+    return v if num_buckets is None else v % np.uint32(num_buckets)
+
+
 def check_hash_invariants(snap: dict, hp: BFHashParams) -> None:
     """CUDASceneRepHashSDF::debugHash (h:179-314): no duplicate blocks, heap and table partition the slots,
     every chain entry reachable from its home bucket within the list limit, all mutexes released."""
@@ -169,8 +177,7 @@ def check_hash_invariants(snap: dict, hp: BFHashParams) -> None:
     assert np.all(snap["mutex"] == -2), "bucket mutex left locked"
     # reachability
     total = hp.m_hashNumBuckets * BF_HASH_BUCKET_SIZE
-    p = pos.astype(np.uint32)
-    hv = ((p[:, 0] * np.uint32(73856093)) ^ (p[:, 1] * np.uint32(19349669)) ^ (p[:, 2] * np.uint32(83492791))) % np.uint32(hp.m_hashNumBuckets)
+    hv = block_hash(pos, hp.m_hashNumBuckets)
     for idx, hb in zip(used, hv.astype(np.int64)):
         if idx // BF_HASH_BUCKET_SIZE == hb:
             continue

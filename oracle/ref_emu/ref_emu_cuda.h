@@ -46,10 +46,6 @@ static inline void emu_sincosf(float a, float* s, float* c) { *s = sinf(a); *c =
 static inline float __fdividef(float a, float b) { return a / b; }
 static inline float rsqrt(float x) { return 1.0f / sqrtf(x); }
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
-static inline int atomicAdd(int* p, int v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const int o = *p; *p = o + v; return o; }
-static inline int atomicCAS(int* p, int cmp, int v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const int o = *p; if (o == cmp) *p = v; return o; }
-static inline int atomicExch(int* p, int v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const int o = *p; *p = v; return o; }
-static inline unsigned atomicSub(unsigned* p, unsigned v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const unsigned o = *p; *p = o - v; return o; }
 static inline uchar3 make_uchar3(float x, float y, float z) { return { (unsigned char)x, (unsigned char)y, (unsigned char)z }; }     // in-range values: truncation, as cvt.rzi
 enum { cudaTextureType1D = 1, cudaTextureType2D = 2 };
 static inline float __shfl_down(float v, int d, int = 32) { return __shfl_down_sync(0xFFFFFFFFu, v, d); }

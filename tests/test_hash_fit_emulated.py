@@ -3,30 +3,18 @@ against tests/cuda_emu (one OS thread per CUDA thread, atomics under a lock) and
 function; the refusals of bfTsdfCountBlocks / bfTsdfBlockKeyLoad / bfTsdfBlockKeyMerge in a process that sees no CUDA device; and
 fuse.fit_hash_params' bucket sequence and byte accounting on synthetic counts."""
 import ctypes as C
-import json
-import os
-import shutil
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 from bundlefusion_b200 import _capi as capi
 from bundlefusion_b200 import fuse
+from oracle import oracle as orc
+from tests.cuda_emu import build_emulated, run_without_device
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIM = 1 << 20
 
-_SRC = r'''
-#include "%(emu)s"
-static inline unsigned long long atomicCAS(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
-    std::lock_guard<std::mutex> lk(emu::g_atomic); const unsigned long long o = *p; if (o == cmp) *p = v; return o;
-}
-static inline unsigned atomicMax(unsigned* p, unsigned v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const unsigned o = *p; if (v > o) *p = v; return o; }
-static inline unsigned long long __ldcg(const unsigned long long* p) { std::lock_guard<std::mutex> lk(emu::g_atomic); return *p; }
-#include "tsdf_keys.cuh"
+_GLUE = r'''
 extern "C" void emu_bucket_load(const unsigned long long* keys, unsigned n, unsigned numBuckets, unsigned* load, unsigned* out, unsigned grid, unsigned block) {
     EMU_LAUNCH(bf::bucket_load_kernel, grid, block, keys, n, numBuckets, load, out);
 }
@@ -39,17 +27,7 @@ extern "C" unsigned long long emu_pack(int x, int y, int z) { return bf::pack_bl
 
 @pytest.fixture(scope="module")
 def emu():
-    d = tempfile.mkdtemp(prefix="bf_hashfit_emu_")
-    try:
-        cpp = os.path.join(d, "keys_emu.cpp")
-        open(cpp, "w").write(_SRC % {"emu": os.path.join(ROOT, "tests", "cuda_emu", "cuda_emu.h")})
-        so = os.path.join(d, "libkeys_emu.so")
-        r = subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-I", os.path.join(ROOT, "tests", "cuda_emu"),
-                            "-I", os.path.join(ROOT, "bundlefusion_b200", "csrc"), cpp, "-o", so], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        L = C.CDLL(so)
-    finally:
-        shutil.rmtree(d, ignore_errors=True)
+    L = build_emulated("tsdf_keys.cuh", 0, glue=_GLUE)
     vp, u = C.c_void_p, C.c_uint
     L.emu_bucket_load.argtypes = [vp, u, u, vp, vp, u, u]
     L.emu_merge.argtypes = [vp, u, vp, vp, u, u, u]
@@ -63,15 +41,8 @@ def pack(pos):
     return (np.uint64(1) << np.uint64(63)) | (p[:, 0].astype(np.uint64) << np.uint64(42)) | (p[:, 1].astype(np.uint64) << np.uint64(21)) | p[:, 2].astype(np.uint64)
 
 
-def hash_pos(pos, buckets):
-    """VoxelUtilHashSDF.h:226-234 in uint32 arithmetic, as hash_pos"""
-    p = np.asarray(pos, np.int64).reshape(-1, 3).astype(np.uint32)
-    v = (p[:, 0] * np.uint32(73856093)) ^ (p[:, 1] * np.uint32(19349669)) ^ (p[:, 2] * np.uint32(83492791))
-    return v % np.uint32(buckets)
-
-
 def expected_load(pos, buckets):
-    load = np.bincount(hash_pos(pos, buckets).astype(np.int64), minlength=buckets)
+    load = np.bincount(orc.block_hash(pos, buckets).astype(np.int64), minlength=buckets)
     return load, int(load.max()) if len(pos) else 0, int(np.maximum(load - capi.BF_HASH_BUCKET_SIZE, 0).sum())
 
 
@@ -113,7 +84,7 @@ def test_bucket_load_at_four_and_five_keys_per_bucket(emu):
     B = 101
     rng = np.random.default_rng(7)
     cand = _random_positions(rng, 20000, 1 << 12)
-    h = hash_pos(cand, B)
+    h = orc.block_hash(cand, B)
     by = [cand[h == b] for b in range(B)]
     four = np.concatenate([by[b][:4] for b in range(0, 40)])
     five = np.concatenate([by[b][:5] for b in range(40, 43)])
@@ -207,10 +178,7 @@ print(json.dumps(out))
 def test_count_and_load_refusals_enqueue_nothing():
     """each malformed call returns cudaErrorInvalidValue (1) before any CUDA call: run in a child process that sees no CUDA device, where a call
     that went on to the runtime would fail with another code (or touch the fake pointers)"""
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    r = subprocess.run([sys.executable, "-c", _REFUSALS, ROOT], capture_output=True, text=True, env=env, cwd=ROOT, timeout=300)
-    assert r.returncode == 0, r.stderr[-3000:]
-    out = json.loads(r.stdout.strip().splitlines()[-1])
+    out = run_without_device(_REFUSALS)
     assert out == {k: 1 for k in out}, out
 
 
@@ -281,9 +249,7 @@ def test_fit_without_a_cap_stops_at_the_default_buckets_per_block():
     """blocks of a surface-like lattice whose 32-bit hash values coincide five or more at a time: no bucket count separates them, the default
     cap ends the search and the overflow that remains is reported"""
     g = np.stack(np.meshgrid(np.arange(-300, 300), np.arange(-300, 300), np.arange(-2, 2), indexing="ij"), -1).reshape(-1, 3)
-    p = g.astype(np.uint32)
-    v = (p[:, 0] * np.uint32(73856093)) ^ (p[:, 1] * np.uint32(19349669)) ^ (p[:, 2] * np.uint32(83492791))
-    _, inv, cnt = np.unique(v, return_inverse=True, return_counts=True)
+    _, inv, cnt = np.unique(orc.block_hash(g), return_inverse=True, return_counts=True)
     pos = g[cnt[inv] >= 5]
     floor = int(np.maximum(cnt - 4, 0).sum())
     assert floor > 0 and len(pos) > 0

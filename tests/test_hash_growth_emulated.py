@@ -3,42 +3,21 @@ OS thread per CUDA thread, atomics under a lock), with the source table built by
 clustered blocks in a table small enough for overflow lists, freed holes, a last list that holds a freed block; rehashed into a larger, a
 same-size and a smaller table.  Also the refusals of bfTsdfRehash in a process that sees no CUDA device, and the frame loop's growth-size rule."""
 import ctypes as C
-import json
-import os
-import shutil
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 from bundlefusion_b200 import _capi as capi
 from bundlefusion_b200.scene_rep import default_hash_params
+from oracle import oracle as orc
+from tests.cuda_emu import build_emulated, run_without_device
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FREE, LIST_LIMIT = capi.BF_FREE_ENTRY, 7
+# the counter layout of csrc/tsdf_shared.cuh (pinned by test_counter_layout_is_the_librarys)
 CTR_HIGH_WATER, CTR_E, CTR_FREED, CTR_HEAP_FAIL, CTR_DROPPED, CTR_SET1, SET_COUNT, CTR_NUM = 0, 3, 8, 9, 10, 24, 0, 32
 VEC = 512 * 3                                              # 32-bit words per voxel block
 
-_SRC = r'''
-#include "%(emu)s"
-#include <thread>
-static inline unsigned long long atomicCAS(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
-    std::lock_guard<std::mutex> lk(emu::g_atomic); const unsigned long long o = *p; if (o == cmp) *p = v; return o;
-}
-static inline unsigned long long __ldcg(const unsigned long long* p) { std::lock_guard<std::mutex> lk(emu::g_atomic); return *p; }
-static inline int atomicCAS(int* p, int cmp, int v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const int o = *p; if (o == cmp) *p = v; return o; }
-static inline int atomicExch(int* p, int v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const int o = *p; *p = v; return o; }
-static inline unsigned atomicSub(unsigned* p, unsigned v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const unsigned o = *p; *p = o - v; return o; }
-static inline unsigned atomicMax(unsigned* p, unsigned v) { std::lock_guard<std::mutex> lk(emu::g_atomic); const unsigned o = *p; if (v > o) *p = v; return o; }
-static inline int __ldcg(const int* p) { std::lock_guard<std::mutex> lk(emu::g_atomic); return *p; }
-static inline unsigned __ldcg(const unsigned* p) { std::lock_guard<std::mutex> lk(emu::g_atomic); return *p; }
-static inline void __stcg(int* p, int v) { std::lock_guard<std::mutex> lk(emu::g_atomic); *p = v; }
-static inline void __threadfence() { std::atomic_thread_fence(std::memory_order_seq_cst); }
-static inline void __nanosleep(unsigned) { std::this_thread::yield(); }
-static inline unsigned __shfl_sync(unsigned m, unsigned v, int src) { return (unsigned)__shfl_sync(m, (int)v, src); }
-#include "tsdf_hash.cuh"
+_GLUE = r'''
 using namespace bf;
 static void insert_kernel(BFHashDataStruct hd, BFHashParams hp, int4* slotInfo, unsigned* ctrs, const int* pos, unsigned n) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -62,33 +41,29 @@ extern "C" void emu_list(const BFHashDataStruct* src, const BFHashDataStruct* ds
                          const unsigned* slotMap, const unsigned char* srcFlags, unsigned char* dstFlags, unsigned grid, unsigned block) {
     EMU_LAUNCH(rehash_list_kernel, grid, block, *src, *dst, srcCtrs, dstCtrs, set, dstSlotInfo, slotMap, srcFlags, dstFlags);
 }
+extern "C" void emu_counter_layout(unsigned* out) {
+    const unsigned v[] = { CTR_HIGH_WATER, CTR_E, CTR_FREED, CTR_HEAP_FAIL, CTR_DROPPED, CTR_SET1, SET_COUNT, CTR_NUM };
+    memcpy(out, v, sizeof v);
+}
 '''
 
 
 @pytest.fixture(scope="module")
 def emu():
-    d = tempfile.mkdtemp(prefix="bf_rehash_emu_")
-    try:
-        cpp = os.path.join(d, "rehash_emu.cpp")
-        open(cpp, "w").write(_SRC % {"emu": os.path.join(ROOT, "tests", "cuda_emu", "cuda_emu.h")})
-        so = os.path.join(d, "librehash_emu.so")
-        r = subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-I", os.path.join(ROOT, "tests", "cuda_emu"),
-                            "-I", os.path.join(ROOT, "bundlefusion_b200", "csrc"), cpp, "-o", so], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        L = C.CDLL(so)
-    finally:
-        shutil.rmtree(d, ignore_errors=True)
+    L = build_emulated("tsdf_hash.cuh", 0, glue=_GLUE)
     vp, u = C.c_void_p, C.c_uint
     L.emu_insert.argtypes = [vp, vp, vp, vp, vp, u]
     L.emu_delete.argtypes = [vp, vp, vp, vp, u]
     L.emu_rehash.argtypes = [vp] * 11 + [u]
     L.emu_list.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, u, u]
+    L.emu_counter_layout.argtypes = [vp]
     return L
 
 
-def hash_pos(pos, buckets):
-    p = np.asarray(pos, np.int64).reshape(-1, 3).astype(np.uint32)
-    return ((p[:, 0] * np.uint32(73856093)) ^ (p[:, 1] * np.uint32(19349669)) ^ (p[:, 2] * np.uint32(83492791))) % np.uint32(buckets)
+def test_counter_layout_is_the_librarys(emu):
+    got = np.zeros(8, np.uint32)
+    emu.emu_counter_layout(got.ctypes.data)
+    assert got.tolist() == [CTR_HIGH_WATER, CTR_E, CTR_FREED, CTR_HEAP_FAIL, CTR_DROPPED, CTR_SET1, SET_COUNT, CTR_NUM]
 
 
 class Table:
@@ -162,7 +137,7 @@ def _source(L, kind, seed):
 def _reachable(t, p):
     """find_entry's rule: the home bucket, then the list hanging off its last entry, within the list limit"""
     B = t.hp.m_hashNumBuckets
-    h = int(hash_pos(p, B)[0])
+    h = int(orc.block_hash(p, B)[0])
     for j in range(4):
         if tuple(t.hash[h * 4 + j, :3]) == p and t.hash[h * 4 + j, 3] != FREE:
             return h * 4 + j
@@ -279,10 +254,7 @@ def test_rehash_refusals_enqueue_nothing():
     """each malformed call returns cudaErrorInvalidValue (1) before any CUDA call, in a child process that sees no CUDA device, and names the
     check that refused it.  That nothing is written to dst, and the refusal of a dst heap smaller than src's live blocks (which needs a read of
     src), are checked on real tables on the GPU (tests/test_hash_growth_gpu.py)."""
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    r = subprocess.run([sys.executable, "-c", _REFUSALS, ROOT], capture_output=True, text=True, env=env, cwd=ROOT, timeout=300)
-    assert r.returncode == 0, r.stderr[-3000:]
-    out = json.loads(r.stdout.strip().splitlines()[-1])
+    out = run_without_device(_REFUSALS)
     assert all(rc == 1 for rc, _ in out.values()), out
     # each case is refused by its own check: a case whose check were missing would fall through to a later one and report that one's reason
     assert {k: msg for k, (_, msg) in out.items()} == {k: "bfTsdfRehash: " + why for k, why in _REASONS.items()}, out

@@ -2,18 +2,13 @@
 lattices and extreme values that test_sift_match_sweeps_gpu.py sends to both CUDA sweeps, and at sizes up to 4096 where the reference's 32
 lanes hold many positions each; and bfSiftMatchBatch's host-side refusal of descriptor arrays that are not 16-byte aligned.  No GPU."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import oracle as orc
 from tests import _sift_cases as sc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.cuda_emu import run_without_device
 
 
 def assert_oracle_is_closed_form(d1, d2, distmax, ratiomax, what=""):
@@ -162,10 +157,7 @@ print(json.dumps(out))
 def test_misaligned_descriptor_arrays_are_refused_on_the_host():
     """a live job whose d_des1 or d_des2 is 1, 4 or 8 bytes past a 16-byte boundary makes bfSiftMatchBatch return cudaErrorInvalidValue before
     any CUDA call; empty jobs (NULL or misaligned pointers, never read) next to a live aligned one are not refused by that check"""
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    r = subprocess.run([sys.executable, "-c", _CHILD, ROOT], env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr
-    out = json.loads(r.stdout.strip().splitlines()[-1])
+    out = run_without_device(_CHILD)
     for k, rc in out.items():
         if k == "empty_null_next_to_aligned":
             assert rc != 1, (k, rc)                      # goes on to the CUDA runtime, which has no device here

@@ -5,11 +5,6 @@ kernel's LOGIC without a GPU: affine voxel -> camera chain, pixel / truncation d
 blend, de-integration rounding, the fused old-pose / new-pose pass, live-voxel and U counters.  TEST INFRASTRUCTURE around a product source;
 the GPU statement is tests/test_tsdf_fast_gpu.py."""
 import ctypes as C
-import os
-import re
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -18,29 +13,13 @@ from bundlefusion_b200 import _capi as capi
 from bundlefusion_b200 import synth
 from bundlefusion_b200.scene_rep import camera_params, default_hash_params, set_pose
 from oracle import oracle as orc
+from tests.cuda_emu import build_emulated
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = np.float32
 
-_PRE = r'''
-#include "%(emu)s"
-static inline unsigned __byte_perm(unsigned x, unsigned y, unsigned s) {
-    const unsigned long long v = ((unsigned long long)y << 32) | x; unsigned r = 0;
-    for (int i = 0; i < 4; ++i) r |= (unsigned)((v >> (8 * ((s >> (4 * i)) & 7))) & 0xff) << (8 * i);
-    return r;
-}
-static inline unsigned __umulhi(unsigned a, unsigned b) { return (unsigned)(((unsigned long long)a * b) >> 32); }
-static inline int atomicAdd(int* p, int v) { const int o = *p; *p = o + v; return o; }
-static inline unsigned long long atomicAdd(unsigned long long* p, unsigned long long v) { const unsigned long long o = *p; *p = o + v; return o; }
-static inline unsigned warp_sum_u(unsigned v) { return v; }
-#define BF_CHECK(e) do { int _e = (int)(e); if (_e) return _e; } while (0)
-#define BF_EMU_SEQUENTIAL 1
-template <class K, class A> static void seq_launch(K kernel, unsigned grid, unsigned block, const A& a) {
-    emu::g_bar.n = 1; gridDim = dim3(grid); blockDim = dim3(block);
-    for (unsigned b = 0; b < grid; ++b) for (unsigned t = 0; t < block; ++t) { blockIdx = { b, 0, 0 }; threadIdx = { t, 0, 0 }; kernel(a); }
-}
-'''
-_POST = r'''
+# the glue of both stencil test files (this one and tests/test_tsdf_integrate_batch_emulated.py); emu_reintegrate_multi with hpOld NULL is
+# the integration batch
+_GLUE = r'''
 extern "C" int emu_integrate_fast(const BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, const float* depth, const void* color,
                                   int deIntegrate, unsigned count, unsigned* ctrs, int* live, int grid) {
     return bf::launch_integrate_fast(hd, hp, cp, depth, color, deIntegrate != 0, false, count, ctrs, live, nullptr, bf::CTR_SET0, grid, nullptr);
@@ -52,34 +31,24 @@ extern "C" int emu_reintegrate_fast(const BFHashDataStruct* hd, const BFHashPara
 extern "C" int emu_reintegrate_multi(const BFHashDataStruct* hd, const BFHashParams* hpOld, const BFHashParams* hpNew, int nOps, const BFDepthCameraParams* cp,
                                      const float* const* depth, const void* const* color, const void* workA, const void* workB, const unsigned* maskA, const unsigned* maskB, unsigned workCap, unsigned* ctrs, int* live, int grid) {
     bf::BFMultiOpDesc d[BF_MULTI_MAX_OPS];
-    for (int k = 0; k < nOps; ++k) { d[k].hpOld = hpOld + k; d[k].hpNew = hpNew + k; d[k].depth = depth[k]; d[k].color = color[k]; }
+    for (int k = 0; k < nOps; ++k) { d[k].hpOld = hpOld ? hpOld + k : nullptr; d[k].hpNew = hpNew + k; d[k].depth = depth[k]; d[k].color = color[k]; }
     return bf::launch_reintegrate_multi_fast(hd, d, nOps, cp, (const int4*)workA, (const int4*)workB, maskA, maskB, workCap, bf::CTR_SET0, ctrs, live, grid, nullptr);
 }
 '''
 
 
-@pytest.fixture(scope="module")
-def emu():
-    src = open(os.path.join(ROOT, "bundlefusion_b200", "csrc", "tsdf_fast.cu")).read()
-    src = src.replace('#include "bf_common.cuh"', "")
-    src, n = re.subn(r"(\w+<\d, \w+>)<<<\s*([^,]+),\s*([^,]+),\s*[^,]+,\s*[^>]+>>>\((\w+)\)", r"seq_launch(\1, \2, \3, \4)", src)
-    assert n == 5, n
-    src, n = re.subn(r"stencil_multi_kernel<<<\s*([^,]+),\s*([^,]+),\s*[^,]+,\s*[^>]+>>>\((\w+)\)", r"seq_launch(stencil_multi_kernel, \1, \2, \3)", src)
-    assert n == 1, n
-    d = tempfile.mkdtemp(prefix="bf_fast_emu_")
-    cpp = os.path.join(d, "tsdf_fast_emu.cpp")
-    open(cpp, "w").write(_PRE % {"emu": os.path.join(ROOT, "tests", "cuda_emu", "cuda_emu.h")} + src + _POST)
-    so = os.path.join(d, "libtsdf_fast_emu.so")
-    r = subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-I", os.path.join(ROOT, "tests", "cuda_emu"),
-                        "-I", os.path.join(ROOT, "bundlefusion_b200", "csrc"), cpp, "-o", so], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    L = C.CDLL(so)
-    shutil.rmtree(d, ignore_errors=True)
+def fast_stencil():
+    L = build_emulated("tsdf_fast.cu", 6, glue=_GLUE, sequential=True)
     vp = C.c_void_p
     L.emu_integrate_fast.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_uint, vp, vp, C.c_int]
     L.emu_reintegrate_fast.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int]
     L.emu_reintegrate_multi.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_uint, vp, vp, C.c_int]
     return L
+
+
+@pytest.fixture(scope="module")
+def emu():
+    return fast_stencil()
 
 
 def _compare(a, b, sdf_tol):

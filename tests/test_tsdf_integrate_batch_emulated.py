@@ -3,12 +3,6 @@ CPU -- the same source compiled by g++ against tests/cuda_emu, one CUDA thread a
 on the oracle's host-side voxel hash, against the one-frame fast stencil applied frame by frame: every voxel word, the live-voxel counters and
 U must be identical.  Also the refusals of bfTsdfIntegrateBatch / bfFrameLoopFuse, which return before any CUDA call."""
 import ctypes as C
-import os
-import re
-import shutil
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -17,67 +11,16 @@ from bundlefusion_b200 import _capi as capi
 from bundlefusion_b200 import synth
 from bundlefusion_b200.scene_rep import camera_params, default_hash_params, set_pose
 from oracle import oracle as orc
+from tests.cuda_emu import run_without_device
+from tests.test_tsdf_fast_emulated import fast_stencil
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = np.float32
 W, H = 160, 120
-
-_PRE = r'''
-#include "%(emu)s"
-static inline unsigned __byte_perm(unsigned x, unsigned y, unsigned s) {
-    const unsigned long long v = ((unsigned long long)y << 32) | x; unsigned r = 0;
-    for (int i = 0; i < 4; ++i) r |= (unsigned)((v >> (8 * ((s >> (4 * i)) & 7))) & 0xff) << (8 * i);
-    return r;
-}
-static inline unsigned __umulhi(unsigned a, unsigned b) { return (unsigned)(((unsigned long long)a * b) >> 32); }
-static inline int atomicAdd(int* p, int v) { const int o = *p; *p = o + v; return o; }
-static inline unsigned long long atomicAdd(unsigned long long* p, unsigned long long v) { const unsigned long long o = *p; *p = o + v; return o; }
-static inline unsigned warp_sum_u(unsigned v) { return v; }
-#define BF_CHECK(e) do { int _e = (int)(e); if (_e) return _e; } while (0)
-#define BF_EMU_SEQUENTIAL 1
-template <class K, class A> static void seq_launch(K kernel, unsigned grid, unsigned block, const A& a) {
-    emu::g_bar.n = 1; gridDim = dim3(grid); blockDim = dim3(block);
-    for (unsigned b = 0; b < grid; ++b) for (unsigned t = 0; t < block; ++t) { blockIdx = { b, 0, 0 }; threadIdx = { t, 0, 0 }; kernel(a); }
-}
-'''
-_POST = r'''
-extern "C" int emu_integrate_fast(const BFHashDataStruct* hd, const BFHashParams* hp, const BFDepthCameraParams* cp, const float* depth, const void* color,
-                                  unsigned count, unsigned* ctrs, int* live, int grid) {
-    return bf::launch_integrate_fast(hd, hp, cp, depth, color, false, false, count, ctrs, live, nullptr, bf::CTR_SET0, grid, nullptr);
-}
-extern "C" int emu_integrate_multi(const BFHashDataStruct* hd, const BFHashParams* hp, int nOps, const BFDepthCameraParams* cp, const float* const* depth,
-                                   const void* const* color, const void* workA, const void* workB, const unsigned* maskA, const unsigned* maskB, unsigned workCap,
-                                   unsigned* ctrs, int* live, int grid) {
-    bf::BFMultiOpDesc d[BF_MULTI_MAX_OPS];
-    for (int k = 0; k < nOps; ++k) { d[k].hpOld = nullptr; d[k].hpNew = hp + k; d[k].depth = depth[k]; d[k].color = color[k]; }
-    return bf::launch_reintegrate_multi_fast(hd, d, nOps, cp, (const int4*)workA, (const int4*)workB, maskA, maskB, workCap, bf::CTR_SET0, ctrs, live, grid, nullptr);
-}
-'''
 
 
 @pytest.fixture(scope="module")
 def emu():
-    src = open(os.path.join(ROOT, "bundlefusion_b200", "csrc", "tsdf_fast.cu")).read()
-    src = src.replace('#include "bf_common.cuh"', "")
-    src, n = re.subn(r"(\w+<\d, \w+>)<<<\s*([^,]+),\s*([^,]+),\s*[^,]+,\s*[^>]+>>>\((\w+)\)", r"seq_launch(\1, \2, \3, \4)", src)
-    assert n == 5, n
-    src, n = re.subn(r"stencil_multi_kernel<<<\s*([^,]+),\s*([^,]+),\s*[^,]+,\s*[^>]+>>>\((\w+)\)", r"seq_launch(stencil_multi_kernel, \1, \2, \3)", src)
-    assert n == 1, n
-    d = tempfile.mkdtemp(prefix="bf_intbatch_emu_")
-    try:
-        cpp = os.path.join(d, "tsdf_intbatch_emu.cpp")
-        open(cpp, "w").write(_PRE % {"emu": os.path.join(ROOT, "tests", "cuda_emu", "cuda_emu.h")} + src + _POST)
-        so = os.path.join(d, "libtsdf_intbatch_emu.so")
-        r = subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-I", os.path.join(ROOT, "tests", "cuda_emu"),
-                            "-I", os.path.join(ROOT, "bundlefusion_b200", "csrc"), cpp, "-o", so], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        L = C.CDLL(so)
-    finally:
-        shutil.rmtree(d, ignore_errors=True)
-    vp = C.c_void_p
-    L.emu_integrate_fast.argtypes = [vp, vp, vp, vp, vp, C.c_uint, vp, vp, C.c_int]
-    L.emu_integrate_multi.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_uint, vp, vp, C.c_int]
-    return L
+    return fast_stencil()
 
 
 class _Scene:
@@ -107,7 +50,7 @@ class _Scene:
         o.L.orc_tsdf_alloc(C.byref(o.hd), C.byref(o.hp), d, C.byref(self.cam))
         n = o.L.orc_tsdf_compactify(C.byref(o.hd), C.byref(o.hp), C.byref(self.cam))
         self.ctrs[16:24] = 0
-        assert self.L.emu_integrate_fast(C.byref(o.hd), C.byref(o.hp), C.byref(self.cam), d.ctypes.data, c.ctypes.data, n, self.ctrs.ctypes.data,
+        assert self.L.emu_integrate_fast(C.byref(o.hd), C.byref(o.hp), C.byref(self.cam), d.ctypes.data, c.ctypes.data, 0, n, self.ctrs.ctypes.data,
                                          self.live.ctypes.data, 3) == 0
         return int(self.ctrs[20]) | (int(self.ctrs[21]) << 32)
 
@@ -145,8 +88,8 @@ class _Scene:
         dptr = (C.c_void_p * n)(*[f[0].ctypes.data for f in frames]); cptr = (C.c_void_p * n)(*[f[1].ctypes.data for f in frames])
         self.ctrs[16:24] = 0
         self.ctrs[16] = len(rows); self.ctrs[17] = len(lay[3]); self.ctrs[18] = len(lay[2]); self.ctrs[22] = len(lay[1]); self.ctrs[23] = len(lay[0])
-        assert self.L.emu_integrate_multi(C.byref(o.hd), C.addressof(hps), n, C.byref(self.cam), C.addressof(dptr), C.addressof(cptr), WA.ctypes.data,
-                                          WB.ctypes.data, MA.ctypes.data, MB.ctypes.data, cap, self.ctrs.ctypes.data, self.live.ctypes.data, 5) == 0
+        assert self.L.emu_reintegrate_multi(C.byref(o.hd), None, C.addressof(hps), n, C.byref(self.cam), C.addressof(dptr), C.addressof(cptr), WA.ctypes.data,
+                                            WB.ctypes.data, MA.ctypes.data, MB.ctypes.data, cap, self.ctrs.ctypes.data, self.live.ctypes.data, 5) == 0
         return int(self.ctrs[20]) | (int(self.ctrs[21]) << 32), epoch
 
 
@@ -212,9 +155,5 @@ print(json.dumps(out))
 def test_integration_batch_refusals_enqueue_nothing():
     """each malformed call returns cudaErrorInvalidValue (1) before any CUDA call: run in a child process that sees no CUDA device, where a call
     that went on to the runtime would fail with another code (or touch the fake pointers)"""
-    import json
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    r = subprocess.run([sys.executable, "-c", _REFUSALS, ROOT], capture_output=True, text=True, env=env, cwd=ROOT, timeout=300)
-    assert r.returncode == 0, r.stderr[-3000:]
-    out = json.loads(r.stdout.strip().splitlines()[-1])
+    out = run_without_device(_REFUSALS)
     assert out == {k: 1 for k in out}, out
