@@ -137,7 +137,8 @@ class BFRayCastData(C.Structure):
 MARCHINGCUBES_SYMBOLS = ["resetMarchingCubesCUDA", "extractIsoSurfaceCUDA", "bfMarchingCubesExtract", "bfMarchingCubesCreate", "bfMarchingCubesDestroy",
                          "bfMarchingCubesExtractIsoSurface", "bfMarchingCubesClearMeshBuffer", "bfMarchingCubesGetSoup", "bfMarchingCubesSaveMesh",
                          "bfMeshMergeCloseVertices", "bfMeshRemoveDuplicateFaces", "bfMeshSavePly", "bfMarchingCubesCount", "bfMarchingCubesExtractRange",
-                         "bfMarchingCubesExtractIsoSurfaceWhole", "bfMarchingCubesGetLastExtraction"]
+                         "bfMarchingCubesExtractIsoSurfaceWhole", "bfMarchingCubesGetLastExtraction", "bfMeshApplyTransform", "bfMeshWeldWorkspaceBytes",
+                         "bfMeshWeld"]
 BF_MC_CHUNK_SLOTS = 512                  # hash slots per chunk of the count pass and of bfMarchingCubesExtractRange
 
 
@@ -157,6 +158,12 @@ class BFMarchingCubesWholeInfo(C.Structure):
     """include/bf_marchingcubes.h: what bfMarchingCubesExtractIsoSurfaceWhole did, 40 bytes"""
     _fields_ = [("trianglesCounted", C.c_uint64), ("trianglesExtracted", C.c_uint64), ("chunks", C.c_uint32), ("parts", C.c_uint32),
                 ("largestPart", C.c_uint32), ("bufferTriangles", C.c_uint32), ("bufferEnlarged", C.c_uint32), ("hostSyncs", C.c_uint32)]
+
+
+class BFMeshWeldInfo(C.Structure):
+    """include/bf_marchingcubes.h: what bfMeshWeld did, 56 bytes"""
+    _fields_ = [("trianglesIn", C.c_uint64), ("verticesOut", C.c_uint64), ("degenerateFaces", C.c_uint64), ("duplicateFaces", C.c_uint64),
+                ("facesOut", C.c_uint64), ("cells", C.c_uint32), ("rounds", C.c_uint32), ("hostSyncs", C.c_uint32)]
 
 
 CACHE_SYMBOLS = ["bfCacheStoreFrame"]

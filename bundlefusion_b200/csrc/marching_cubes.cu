@@ -376,6 +376,17 @@ static int save_ply(const char* filename, const float* pos, const float* col, si
     return (fclose(f) == 0 && ok) ? 0 : 1;
 }
 
+// MeshData::applyTransform: p' = M * (p, 1), de-homogenised (mLib core-math/matrix4x4.h:479-488)
+static void apply_transform(float* positions, size_t numV, const float* transform) {
+    for (size_t v = 0; v < numV; ++v) {
+        float* p = &positions[3 * v];
+        const float x = p[0], y = p[1], z = p[2];
+        float r[4];
+        for (int k = 0; k < 4; ++k) r[k] = transform[4 * k] * x + transform[4 * k + 1] * y + transform[4 * k + 2] * z + transform[4 * k + 3];
+        p[0] = r[0] / r[3]; p[1] = r[1] / r[3]; p[2] = r[2] / r[3];
+    }
+}
+
 static bool file_exists(const std::string& p) { struct stat st; return stat(p.c_str(), &st) == 0; }
 
 }  // namespace bf
@@ -605,6 +616,12 @@ BF_API int bfMeshSavePly(const char* filename, const float* positions, const flo
     return save_ply(filename, positions, colors, numVertices, faces, numFaces);
 }
 
+BF_API int bfMeshApplyTransform(float* positions, size_t numVertices, const float* transform) {
+    if ((!positions && numVertices) || !transform) return 1;
+    apply_transform(positions, numVertices, transform);
+    return 0;
+}
+
 BF_API int bfMarchingCubesSaveMesh(BFMarchingCubes* mc, const char* filename, const float* transform, int overwrite, char* actualPath, size_t actualPathCapacity) {
     if (!mc || !filename) return 1;
     std::string name = filename;
@@ -633,15 +650,7 @@ BF_API int bfMarchingCubesSaveMesh(BFMarchingCubes* mc, const char* filename, co
     for (size_t i = 0; i < faces.size(); ++i) faces[i] = (uint32_t)i;
     merge_close_vertices(mc->positions, mc->colors, faces, 0.00001f);
     remove_duplicate_faces(faces);
-    if (transform) {                                                     // MeshData::applyTransform: p' = M * (p, 1), de-homogenised (mLib core-math/matrix4x4.h:479-488)
-        for (size_t v = 0; v < mc->positions.size() / 3; ++v) {
-            float* p = &mc->positions[3 * v];
-            const float x = p[0], y = p[1], z = p[2];
-            float r[4];
-            for (int k = 0; k < 4; ++k) r[k] = transform[4 * k] * x + transform[4 * k + 1] * y + transform[4 * k + 2] * z + transform[4 * k + 3];
-            p[0] = r[0] / r[3]; p[1] = r[1] / r[3]; p[2] = r[2] / r[3];
-        }
-    }
+    if (transform) apply_transform(mc->positions.data(), mc->positions.size() / 3, transform);
     const int rc = save_ply(name.c_str(), mc->positions.data(), mc->colors.empty() ? nullptr : mc->colors.data(), mc->positions.size() / 3, faces.data(), faces.size() / 3);
     if (actualPath && actualPathCapacity) { strncpy(actualPath, name.c_str(), actualPathCapacity - 1); actualPath[actualPathCapacity - 1] = 0; }
     bfMarchingCubesClearMeshBuffer(mc);

@@ -233,15 +233,26 @@ def fit_hash_params(base_hp, voxel_size: float, counter, max_table_bytes: int | 
     return hp, report
 
 
-def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6_000_000, whole: bool = False) -> dict:
+def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6_000_000, whole: bool = False, device_mesh: bool = False) -> dict:
     """iso-surface of a scene (threshold 10 x voxel, the reference's s_SDFMarchingCubeThreshFactor) saved as PLY.  Returns {"triangles" (in the
     mesh), "triangles_found" (the cells produced), "triangles_dropped" (found - kept: what a full buffer of max_num_triangles lost), "mesh_path"}.
     whole=True extracts through CUDAMarchingCubesHashSDF.extractIsoSurfaceWhole -- counted first, then in parts that fit the buffer, so nothing
-    is dropped -- and adds its report under "mesh"."""
+    is dropped -- and adds its report under "mesh".
+    device_mesh=True extracts the whole soup into device memory (CUDAMarchingCubesHashSDF.extractSoup) and cleans it up there (weld): the same
+    PLY as saveMesh, written from the device mesh; the weld's report and the bytes the path holds at once go under "mesh".  It trades device
+    memory (soup, workspace and outputs together) for time, so it is an option."""
+    if whole and device_mesh:
+        raise ValueError("mesh_scene: whole and device_mesh are two different paths; pick one")
     hp = scene.m_hashParams
     mc = CUDAMarchingCubesHashSDF(marching_cubes_params(int(hp.m_hashNumBuckets), float(hp.m_virtualVoxelSize), max_num_triangles), device)
     try:
         out = {}
+        if device_mesh:
+            mesh = mc.extractMesh(scene)
+            n = int(mesh.info["triangles_in"])
+            out.update(mesh={**mesh.info, "peak_device_bytes": mesh.info.pop("device_bytes")}, triangles=n, triangles_found=n, triangles_dropped=0,
+                       mesh_path=mesh.save_ply(ply_path))
+            return out
         if whole:
             out["mesh"] = mc.extractIsoSurfaceWhole(scene)
         else:
@@ -255,7 +266,8 @@ def mesh_scene(scene, ply_path: str, device="cuda:0", max_num_triangles: int = 6
 
 def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: float = 0.004, poses="recorded", hash_buckets: int | None = None,
                    sdf_blocks: int | None = None, device="cuda:0", max_frames: int | None = None, scene: CUDASceneRepHashSDF | None = None,
-                   max_num_triangles: int = 6_000_000, fit_hash: bool = False, max_table_bytes: int | None = None, whole_mesh: bool = False) -> dict:
+                   max_num_triangles: int = 6_000_000, fit_hash: bool = False, max_table_bytes: int | None = None, whole_mesh: bool = False,
+                   device_mesh: bool = False) -> dict:
     """Fuses a .sens recording along fixed camera-to-world poses -- "recorded" (the poses stored with the frames) or an array [n, 4, 4] --
     into a voxel hash of voxel_size (or into ``scene``, a reset CUDASceneRepHashSDF), with no bundling.  Frames whose pose is not finite are
     skipped.  Returns {"frames", "fused", "skipped", "batches", "inserts_dropped" (block inserts the hash had no room for), "heap_free",
@@ -265,8 +277,11 @@ def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: floa
     also holds "blocks_counted", "buckets", "predicted_overflow" (0 unless max_table_bytes was too small to avoid overflow) and the whole
     report under "fit".  fit_hash excludes hash_buckets, sdf_blocks and scene.
     The mesh: "triangles_found" and "triangles_dropped" as mesh_scene reports them; whole_mesh=True meshes through mesh_scene(whole=True), which
-    drops nothing however small max_num_triangles is, and adds its report under "mesh"."""
+    drops nothing however small max_num_triangles is, and adds its report under "mesh"; device_mesh=True meshes through
+    mesh_scene(device_mesh=True)."""
     import torch
+    if whole_mesh and device_mesh:
+        raise ValueError("whole_mesh and device_mesh are two different mesh paths: pick one")
     if fit_hash and (hash_buckets is not None or sdf_blocks is not None or scene is not None):
         raise ValueError("fit_hash sizes the hash itself: pass no hash_buckets, sdf_blocks or scene")
     dev = torch.device(device)
@@ -326,7 +341,7 @@ def fuse_recording(sens_path: str, ply_path: str | None = None, voxel_size: floa
             out.update(blocks_counted=fit["blocks_counted"], buckets=fit["buckets"], predicted_overflow=fit["predicted_overflow"], fit=fit)
         out.update(triangles=0, triangles_found=0, triangles_dropped=0, mesh_path=None, scene=scene)
         if ply_path is not None:
-            out.update(mesh_scene(scene, ply_path, device, max_num_triangles, whole=whole_mesh))
+            out.update(mesh_scene(scene, ply_path, device, max_num_triangles, whole=whole_mesh, device_mesh=device_mesh))
         return out
     finally:
         r.close()

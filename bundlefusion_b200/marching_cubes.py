@@ -37,6 +37,9 @@ def _bind(L):
     L.bfMarchingCubesExtractRange.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp]
     L.bfMarchingCubesExtractIsoSurfaceWhole.argtypes = [vp, vp, vp, vp, vp, C.c_int, vp]
     L.bfMarchingCubesGetLastExtraction.argtypes = [vp, C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
+    L.bfMeshApplyTransform.argtypes = [vp, sz, vp]
+    L.bfMeshWeldWorkspaceBytes.argtypes = [C.c_uint64]; L.bfMeshWeldWorkspaceBytes.restype = sz
+    L.bfMeshWeld.argtypes = [vp, C.c_uint64, C.c_float, vp, sz, vp, vp, vp, vp]
     L._mc_bound = True
     return L
 
@@ -71,6 +74,70 @@ def save_ply(path: str, positions: np.ndarray, colors: np.ndarray | None, faces:
     col = None if colors is None else np.ascontiguousarray(colors, np.float32)
     if L.bfMeshSavePly(path.encode(), pos.ctypes.data, None if col is None else col.ctypes.data, len(pos), f.ctypes.data, len(f)):
         raise OSError(f"bfMeshSavePly({path}) failed")
+
+
+def apply_transform(positions: np.ndarray, transform) -> np.ndarray:
+    """saveMesh's transform (bfMeshApplyTransform): p' = M (p, 1), de-homogenised, M a row-major 4x4; returns a new float32 array"""
+    L = _bind(capi.lib())
+    pos = np.ascontiguousarray(positions, np.float32).copy()
+    t = np.ascontiguousarray(transform, np.float32)
+    if t.shape != (4, 4) or L.bfMeshApplyTransform(pos.ctypes.data, len(pos), t.ctypes.data):
+        raise ValueError("apply_transform: positions [n, 3] and a 4x4 transform")
+    return pos
+
+
+def _weld_report(info) -> dict:
+    return {"triangles_in": int(info.trianglesIn), "vertices_out": int(info.verticesOut), "degenerate_faces": int(info.degenerateFaces),
+            "duplicate_faces": int(info.duplicateFaces), "faces_out": int(info.facesOut), "cells": int(info.cells), "rounds": int(info.rounds),
+            "host_syncs": int(info.hostSyncs)}
+
+
+class Mesh:
+    """an indexed mesh in device memory: positions [V, 3] float32, colors [V, 4] float32 (w = 1), faces [F, 3] int32, and the weld's report"""
+
+    def __init__(self, positions, colors, faces, info: dict):
+        self.positions, self.colors, self.faces, self.info = positions, colors, faces, info
+
+    def save_ply(self, path: str, transform=None) -> str:
+        """the binary PLY saveMesh writes for this mesh (bfMeshSavePly; with transform, bfMeshApplyTransform first); returns path"""
+        pos = self.positions.cpu().numpy()
+        if transform is not None:
+            pos = apply_transform(pos, transform)
+        save_ply(path, pos, self.colors.cpu().numpy(), self.faces.cpu().numpy().view(np.uint32))
+        return path
+
+
+def weld_workspace_bytes(num_triangles: int) -> int:
+    return int(_bind(capi.lib()).bfMeshWeldWorkspaceBytes(int(num_triangles)))
+
+
+def weld(soup, thresh: float = 0.00001) -> Mesh:
+    """saveMesh's clean-up on the device (bfMeshWeld): soup is a contiguous CUDA float32 tensor [T, 3, 6] (per vertex position, colour), as the
+    extraction writes it.  The result equals merge_close_vertices(thresh) + remove_duplicate_faces on the same soup with colours (c, 1), bit for
+    bit.  Runs on the current stream of the soup's device and synchronises once per round of the vertex merge plus once."""
+    import torch
+    if not (isinstance(soup, torch.Tensor) and soup.is_cuda and soup.dtype == torch.float32 and soup.dim() == 3 and tuple(soup.shape[1:]) == (3, 6)
+            and soup.is_contiguous()):
+        raise ValueError("weld: soup must be a contiguous CUDA float32 tensor [T, 3, 6]")
+    L = _bind(capi.lib())
+    dev = soup.device
+    T = int(soup.shape[0])
+    ws_bytes = int(L.bfMeshWeldWorkspaceBytes(T))
+    if T and ws_bytes == 0:
+        raise ValueError(f"weld: {T} triangles: 3T must be below 2^31 (PLY indices are int)")
+    with torch.cuda.device(dev):
+        L.bfSetStream(C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+        pos = torch.empty((3 * T, 3), dtype=torch.float32, device=dev)
+        col = torch.empty((3 * T, 4), dtype=torch.float32, device=dev)
+        faces = torch.empty((T, 3), dtype=torch.int32, device=dev)
+        info = capi.BFMeshWeldInfo()
+        capi.check(L.bfMeshWeld(soup.data_ptr(), T, thresh, ws.data_ptr(), ws_bytes, pos.data_ptr(), col.data_ptr(), faces.data_ptr(), C.byref(info)), "bfMeshWeld")
+        del ws
+        V, F = int(info.verticesOut), int(info.facesOut)
+        out = Mesh(pos[:V].clone(), col[:V].clone(), faces[:F].clone(), _weld_report(info))
+    out.info["device_bytes"] = T * 72 + ws_bytes + 3 * T * (12 + 16) + T * 12              # soup, workspace and outputs: what the weld holds at once
+    return out
 
 
 class CUDAMarchingCubesHashSDF:
@@ -131,6 +198,25 @@ class CUDAMarchingCubesHashSDF:
         return {"triangles_counted": int(info.trianglesCounted), "triangles_extracted": int(info.trianglesExtracted), "chunks": int(info.chunks),
                 "parts": int(info.parts), "largest_part": int(info.largestPart), "buffer_triangles": int(info.bufferTriangles),
                 "buffer_enlarged": bool(info.bufferEnlarged), "host_syncs": int(info.hostSyncs)}
+
+    def extractSoup(self, scene, min_corner=(0.0, 0.0, 0.0), max_corner=(0.0, 0.0, 0.0), box_enabled: bool = False):
+        """the whole triangle soup in device memory: the count pass (read back once), a soup tensor [T, 3, 6] of exactly that size, and one
+        bfMarchingCubesExtractRange over every chunk.  No triangle is dropped; the mesh buffer is not touched."""
+        t = self._torch
+        total, _ = self.count(scene, min_corner, max_corner, box_enabled)
+        soup = t.empty((total, 3, 6), dtype=t.float32, device=self.device)
+        if total:
+            p = self._box_params(scene, min_corner, max_corner, box_enabled)
+            p.m_maxNumTriangles = total
+            n = t.empty(1, dtype=t.int32, device=self.device)
+            self._bind_stream()
+            capi.check(self.lib.bfMarchingCubesExtractRange(C.byref(scene.m_hashData), C.byref(scene.m_hashParams), C.byref(p), 0, num_chunks(p.m_hashNumBuckets),
+                                                            soup.data_ptr(), n.data_ptr()), "bfMarchingCubesExtractRange")
+        return soup
+
+    def extractMesh(self, scene, min_corner=(0.0, 0.0, 0.0), max_corner=(0.0, 0.0, 0.0), box_enabled: bool = False, thresh: float = 0.00001) -> Mesh:
+        """weld(extractSoup(...)): the indexed mesh saveMesh would write, in device memory"""
+        return weld(self.extractSoup(scene, min_corner, max_corner, box_enabled), thresh)
 
     def lastExtraction(self) -> tuple[int, int]:
         """(found, kept) of the last extraction: triangles its cells produced and triangles it appended; found > kept when a full buffer dropped some"""

@@ -10,9 +10,11 @@ the next decoded frame) -> ``CUDAMarchingCubesHashSDF``.  Host glue only; every 
         [--grow-hash MAX_BLOCKS]    start the online hash at --sdf-blocks and let the loop grow it up to MAX_BLOCKS voxel blocks while it scans
         [--device-frames N]         keep N frame slots on the device and every frame in pinned host memory (same results, less device memory)
         [--whole-mesh]              count the mesh's triangles first and extract them in parts that fit the triangle buffer, so none is dropped
+        [--device-mesh]             extract the whole soup into device memory and merge its vertices and faces there (same PLY, more device memory)
 
 The JSON summary always carries "triangles_found" (what the iso-surface's cells produced) and "triangles_dropped" (what a full triangle buffer
-lost: found - kept); with --whole-mesh it is 0, and the extraction's report (parts, buffer, synchronisations) goes under "mesh".
+lost: found - kept); with --whole-mesh it is 0, and the extraction's report (parts, buffer, synchronisations) goes under "mesh"; with
+--device-mesh it is 0 too, and the weld's report (vertices, faces, rounds, synchronisations, peak device bytes) goes under "mesh".
 """
 from __future__ import annotations
 
@@ -40,7 +42,7 @@ class _LoopScene:
 def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", max_frames: int | None = None, hash_buckets: int | None = None,
                 sdf_blocks: int | None = None, max_num_triangles: int = 6_000_000, tweak=None, solve_frames_before_exit: int | None = None,
                 mesh_voxel_size: float | None = None, fit_hash: bool = False, grow_hash: int | None = None,
-                device_frames: int | None = None, whole_mesh: bool = False) -> dict:
+                device_frames: int | None = None, whole_mesh: bool = False, device_mesh: bool = False) -> dict:
     """runs the sequence; returns {"frames", "valid", "keyframes", "trajectory" [n, 4, 4], "mesh_path", "triangles", "status" (per frame)}.
     solve_frames_before_exit=K ends the recording as the reference does (FrameLoop.finish: sparse global solves to past-end turn K, the dense
     global solve at turn K, then re-integration until every frame is fused at its final pose) and adds that call's info under "finish";
@@ -50,7 +52,8 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
     sdf_blocks (default: the loop's) and the loop may grow it up to MAX_BLOCKS voxel blocks (hashMaxSDFBlocks); FrameLoop.hash_growth() goes
     under "hash".  device_frames=N keeps N frame slots on the device over a pinned host store of every frame (deviceFrameSlots); the results
     do not change, and FrameLoop.frame_store() goes under "frame_store".  The mesh adds "triangles_found" and "triangles_dropped"
-    (fuse.mesh_scene); whole_mesh=True extracts it counted and in parts that fit the buffer, dropping nothing, and adds the report under "mesh"."""
+    (fuse.mesh_scene); whole_mesh=True extracts it counted and in parts that fit the buffer, dropping nothing, and adds the report under "mesh";
+    device_mesh=True extracts the whole soup to the device and welds it there (fuse.mesh_scene(device_mesh=True)), report under "mesh"."""
     r = SensorDataReader(sens_path)
     n = len(r) if max_frames is None else min(len(r), max_frames)
     P = fuse.recording_params(r.header, n)
@@ -95,11 +98,11 @@ def reconstruct(sens_path: str, ply_path: str | None = None, device="cuda:0", ma
         scene = CUDASceneRepHashSDF(hp, device)
         out["fuse"] = loop.fuse(scene, n=n)
         if ply_path is not None:
-            out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles, whole=whole_mesh))
+            out.update(fuse.mesh_scene(scene, ply_path, device, max_num_triangles, whole=whole_mesh, device_mesh=device_mesh))
         scene.close()
     elif ply_path is not None:
         # the table the loop holds now: a grown one has more buckets than P.hash
-        out.update(fuse.mesh_scene(_LoopScene(loop), ply_path, device, max_num_triangles, whole=whole_mesh))
+        out.update(fuse.mesh_scene(_LoopScene(loop), ply_path, device, max_num_triangles, whole=whole_mesh, device_mesh=device_mesh))
     if device_frames is not None:
         out["frame_store"] = loop.frame_store()
     loop.close(); r.close()
@@ -158,7 +161,12 @@ def main(argv=None) -> int:
     ap.add_argument("--whole-mesh", action="store_true",
                     help="count the iso-surface's triangles on the device and extract them in parts that fit the triangle buffer, so that none is "
                          "dropped (the JSON summary carries the extraction's report under 'mesh')")
+    ap.add_argument("--device-mesh", action="store_true",
+                    help="extract the whole triangle soup into device memory and merge its vertices and faces there: the same PLY, cleaned up on the device, "
+                         "for the device memory of soup, workspace and mesh at once (the JSON summary carries the weld's report under 'mesh')")
     a = ap.parse_args(argv)
+    if a.whole_mesh and a.device_mesh:
+        ap.error("--whole-mesh and --device-mesh are two different mesh paths: pick one")
     if a.fit_hash and a.poses != "recorded" and a.mesh_voxel_size is None:
         ap.error("--fit-hash sizes a fused hash: use it with --mesh-voxel-size or --poses recorded")
     if a.poses == "recorded":
@@ -166,7 +174,7 @@ def main(argv=None) -> int:
             ap.error("--fit-hash sizes the fused hash itself: drop --hash-buckets / --sdf-blocks")
         voxel = a.mesh_voxel_size if a.mesh_voxel_size is not None else float(default_params(16, 16).hash.m_virtualVoxelSize)
         o = fuse.fuse_recording(a.sens, a.ply, voxel, "recorded", a.hash_buckets, a.sdf_blocks, a.device, a.frames, fit_hash=a.fit_hash,
-                                whole_mesh=a.whole_mesh)
+                                whole_mesh=a.whole_mesh, device_mesh=a.device_mesh)
         o["scene"].close()
         summary = {"frames": o["frames"], "fuse": {k: o[k] for k in ("fused", "skipped", "batches", "inserts_dropped", "heap_free")},
                    "triangles": o["triangles"], "mesh_path": o["mesh_path"], "triangles_found": o["triangles_found"],
@@ -179,7 +187,7 @@ def main(argv=None) -> int:
         return 0
     o = reconstruct(a.sens, a.ply, a.device, a.frames, a.hash_buckets, a.sdf_blocks, solve_frames_before_exit=a.solve_frames_before_exit,
                     mesh_voxel_size=a.mesh_voxel_size, fit_hash=a.fit_hash, grow_hash=a.grow_hash,
-                    device_frames=a.device_frames, whole_mesh=a.whole_mesh)
+                    device_frames=a.device_frames, whole_mesh=a.whole_mesh, device_mesh=a.device_mesh)
     if a.trajectory:
         np.savetxt(a.trajectory, o["trajectory"].reshape(-1, 16))
     summary = {k: o[k] for k in ("frames", "valid", "keyframes", "triangles", "mesh_path", "triangles_found", "triangles_dropped")}

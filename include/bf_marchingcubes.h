@@ -131,6 +131,33 @@ int  bfMarchingCubesSaveMesh(BFMarchingCubes* mc, const char* filename, const fl
 int  bfMeshMergeCloseVertices(float* positions, float* colors, size_t numVertices, uint32_t* faces, size_t numFaces, float thresh, size_t* numVerticesOut, size_t* numFacesOut);
 int  bfMeshRemoveDuplicateFaces(uint32_t* faces, size_t numFaces, size_t* numFacesOut);
 int  bfMeshSavePly(const char* filename, const float* positions, const float* colors /* [n][4] or NULL */, size_t numVertices, const uint32_t* faces, size_t numFaces);
+/* saveMesh's transform (MeshData::applyTransform): p' = M * (p, 1) with M row-major 4x4, de-homogenised, in place on host positions [n][3] */
+int  bfMeshApplyTransform(float* positions, size_t numVertices, const float* transform);
+
+/* ---- the mesh clean-up on the device ----
+ * bfMeshWeld takes a triangle soup in device memory in the extraction's layout (vertex i = soup vertex i, face t = (3t, 3t+1, 3t+2)) and writes
+ * what bfMeshMergeCloseVertices(thresh) followed by bfMeshRemoveDuplicateFaces give on the same soup with colours (c, 1), bit for bit: merged
+ * positions in first-occurrence order, their colours with w = 1, faces in their surviving order.  Vertices no face references are kept.
+ * The result does not depend on thread scheduling.  It runs on the library stream (bfSetStream) and synchronises the host once per round of
+ * the vertex merge plus once at the end (BFMeshWeldInfo.hostSyncs).  The caller owns the workspace (bfMeshWeldWorkspaceBytes, about
+ * 90-150 bytes per triangle) and the outputs, sized for the worst case: positions [3T][3], colours [3T][4], faces [T][3].
+ * Refused before anything is enqueued (cudaErrorInvalidValue, reason in bfGetLastErrorString): a NULL info; NULL pointers when T > 0; thresh
+ * not finite or not > 0; 3T >= 2^31 (PLY indices are int); a workspace smaller than bfMeshWeldWorkspaceBytes(T).
+ * Refused on the device: a position that is not finite, or whose cell index (p / thresh, rounded as the host rounds it) lies outside int32;
+ * the call then returns cudaErrorInvalidValue with *info all zero and nothing written to the outputs. */
+typedef struct BFMeshWeldInfo {
+    uint64_t trianglesIn;                   /* T */
+    uint64_t verticesOut;                   /* merged vertices written to positions / colours */
+    uint64_t degenerateFaces;               /* faces with a repeated index after the merge (removeDegeneratedFaces) */
+    uint64_t duplicateFaces;                /* non-degenerate faces whose vertex set an earlier face has (removeDuplicateFaces) */
+    uint64_t facesOut;                      /* T - degenerateFaces - duplicateFaces */
+    uint32_t cells;                         /* occupied cells of size thresh */
+    uint32_t rounds;                        /* rounds of the vertex merge: 1 + the longest chain of cells that wait for an earlier neighbour */
+    uint32_t hostSyncs;                     /* rounds + 1 */
+} BFMeshWeldInfo;
+size_t bfMeshWeldWorkspaceBytes(uint64_t numTriangles);     /* 0 when 3 * numTriangles >= 2^31 */
+int  bfMeshWeld(const BFMarchingCubesTriangle* d_soup, uint64_t numTriangles, float thresh, void* d_workspace, size_t workspaceBytes,
+                float* d_positions /* [3T][3] */, float* d_colors /* [3T][4] */, uint32_t* d_faces /* [T][3] */, BFMeshWeldInfo* info);
 
 #ifdef __cplusplus
 }
