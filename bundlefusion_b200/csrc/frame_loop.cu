@@ -263,7 +263,7 @@ struct Loop {
     unsigned numFrames = 0;                      // frames received (CUDAImageManager::getCurrFrameNumber() + 1)
     float currIntegrate[16];
     BFTrajectoryManager* tm = nullptr;
-    // scene
+    // scene: the table's buffers are stream-ordered allocations the loop owns (hash_alloc), not the arena's, so that growth can replace them
     BFHashDataStruct hd; BFHashParams hp; BFDepthCameraParams cam;
     // pinned status block
     int* h_pin = nullptr;
@@ -284,8 +284,7 @@ struct Loop {
     bool profile = false; cudaEvent_t stageEv[BF_FRAMELOOP_STAGES + 1] = {}; bool stageHit[BF_FRAMELOOP_STAGES + 1] = {}; double stageMs[BF_FRAMELOOP_STAGES] = {}; unsigned long long profiledSteps = 0;
     // op log (bfFrameLoopSetOpLog): every TSDF op reconstruct() hands to bfTsdfRunOps, with the turn (step or past-end turn, counted from 0) that issued it
     bool opLogOn = false; unsigned turn = 0; std::vector<BFTsdfOp> opLog; std::vector<uint32_t> opLogTurn;
-    // hash growth (bfFrameLoopGetHashGrowth): the table's buffers are stream-ordered allocations the loop owns (not the arena's); h_hashStat
-    // receives {heap counter, heap failures, drops} of the turn statTurn, evHashStat marks its arrival
+    // hash growth (bfFrameLoopGetHashGrowth): h_stat receives {heap counter, heap failures, drops} of the turn statTurn, ev marks its arrival
     struct Growth {
         bool on = false, ceilingReached = false, pending = false, sampled = false;
         unsigned growths = 0, discarded = 0, initBlocks = 0, initBuckets = 0, bucketScale = 1;
@@ -860,9 +859,9 @@ static int optimize_global(Loop& L) {
     return 0;
 }
 
-// ---- hash growth (bf_frameloop.h, bfFrameLoopGetHashGrowth) --------------------------------------------------------------------------
-// the buffers of a voxel hash of hp's sizes, as stream-ordered allocations on the library stream (bfTsdfReset initialises them); the
-// d_hashDecision arrays and the list counter start zeroed, as the arena's do
+// ---- the voxel hash's buffers, and its growth (bf_frameloop.h, bfFrameLoopGetHashGrowth) ----------------------------------------------
+// the buffers of a voxel hash of hp's sizes, as stream-ordered allocations on the library stream (bfTsdfReset initialises them); the heap
+// counter, the d_hashDecision arrays and the list counter start zeroed
 static void hash_free(BFHashDataStruct& hd) {
     void* p[9] = { hd.d_heap, hd.d_heapCounter, hd.d_hashDecision, hd.d_hashDecisionPrefix, hd.d_hash, hd.d_hashCompactified, hd.d_hashCompactifiedCounter,
                    hd.d_SDFBlocks, hd.d_hashBucketMutex };
@@ -881,7 +880,7 @@ static int hash_alloc(BFHashDataStruct& hd, const BFHashParams& hp) {
     for (auto& x : b) {
         cudaError_t e = cudaMallocAsync(x.p, x.bytes, stream());
         if (e == cudaSuccess && x.zero) e = cudaMemsetAsync(*x.p, 0, x.bytes, stream());
-        if (e != cudaSuccess) { set_last_error("frame loop: hash growth allocation", e); hash_free(hd); return (int)e; }
+        if (e != cudaSuccess) { set_last_error("frame loop: hash allocation", e); hash_free(hd); return (int)e; }
     }
     hd.m_bIsOnGPU = 1;
     return 0;
@@ -1046,8 +1045,9 @@ static int bundler_init(Loop& L, Bundler& b, bool isLocal, unsigned maxImages) {
     return 0;
 }
 
-// a growing loop's table, read-back slot and event (bfFrameLoopDestroy, or a failed bfFrameLoopCreate)
-static void release_grown_hash(Loop& L) {
+// the loop's table, and a growing loop's read-back slot and event (bfFrameLoopDestroy, or a failed bfFrameLoopCreate); the table's memory
+// is back with the device when this returns
+static void release_hash(Loop& L) {
     bfTsdfReleaseAux(&L.hd);
     hash_free(L.hd);
     cudaStreamSynchronize(stream());
@@ -1192,24 +1192,13 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
         L.tm = bfTrajectoryCreate(P.maxNumFrames, P.topNActive, P.minPoseDistSqrt);
         // scene representation
         L.hp = P.hash; L.hp.m_hashBucketSize = BF_HASH_BUCKET_SIZE; L.hp.m_SDFBlockSize = BF_SDF_BLOCK_SIZE;
-        const size_t nEntries = (size_t)L.hp.m_hashNumBuckets * BF_HASH_BUCKET_SIZE;
-        memset(&L.hd, 0, sizeof(L.hd));
+        if ((rc = hash_alloc(L.hd, L.hp))) break;
         L.grow.on = P.hashMaxSDFBlocks > L.hp.m_numSDFBlocks && L.hp.m_numSDFBlocks > 0;
-        if (L.grow.on) {                 // a table the loop may replace: its own stream-ordered buffers, a pinned read-back slot and its event
+        if (L.grow.on) {                 // a table the loop may replace: a pinned read-back slot and its event
             L.grow.initBlocks = L.hp.m_numSDFBlocks; L.grow.initBuckets = L.hp.m_hashNumBuckets;
-            if ((rc = hash_alloc(L.hd, L.hp))) break;
             cudaError_t e = cudaMallocHost(&L.grow.h_stat, 4 * sizeof(unsigned));
             if (e == cudaSuccess) e = cudaEventCreateWithFlags(&L.grow.ev, cudaEventDisableTiming);
             if (e != cudaSuccess) { rc = (int)e; break; }
-        } else {
-            L.hd.d_heap = L.A.get<uint32_t>(L.hp.m_numSDFBlocks, false); L.hd.d_heapCounter = L.A.get<uint32_t>(1);
-            L.hd.d_hashDecision = L.A.get<int32_t>(nEntries); L.hd.d_hashDecisionPrefix = L.A.get<int32_t>(nEntries);
-            L.hd.d_hash = L.A.get<BFHashEntry>(nEntries, false); L.hd.d_hashCompactified = L.A.get<BFHashEntry>(nEntries, false);
-            L.hd.d_hashCompactifiedCounter = L.A.get<int32_t>(1);
-            L.hd.d_SDFBlocks = L.A.get<BFVoxel>((size_t)L.hp.m_numSDFBlocks * BF_SDF_BLOCK_VOXELS, false);
-            L.hd.d_hashBucketMutex = L.A.get<int32_t>(L.hp.m_hashNumBuckets, false);
-            L.hd.m_bIsOnGPU = 1;
-            if (L.A.err) { rc = L.A.err; break; }
         }
         memset(&L.cam, 0, sizeof(L.cam));
         // integration camera: depth intrinsics scaled to the integration resolution (CUDAImageManager: m_depthIntrinsics adapted, cpp:60-70)
@@ -1235,7 +1224,7 @@ BF_API int bfFrameLoopCreate(const BFFrameLoopParams* params, BFFrameLoop** out)
         if (L.tm) bfTrajectoryDestroy(L.tm);
         if (L.h_pin) cudaFreeHost(L.h_pin);
         if (L.h_complete) cudaFreeHost(L.h_complete);
-        if (L.grow.on) release_grown_hash(L);
+        release_hash(L);
         frame_store_release(L);
         delete Lp; return rc;
     }
@@ -1249,8 +1238,7 @@ BF_API void bfFrameLoopDestroy(BFFrameLoop* loop) {
     if (L->tsdfStream) cudaStreamSynchronize(L->tsdfStream);
     if (L->featStream) cudaStreamSynchronize(L->featStream);
     cudaStreamSynchronize(stream());
-    bfTsdfReleaseAux(&L->hd);
-    if (L->grow.on) release_grown_hash(*L);
+    release_hash(*L);
     frame_store_release(*L);
     if (L->tsdfStream) cudaStreamDestroy(L->tsdfStream);
     if (L->featStream) cudaStreamDestroy(L->featStream);

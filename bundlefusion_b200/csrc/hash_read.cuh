@@ -1,16 +1,16 @@
 // hash_read.cuh -- read-only access to the hashed TSDF shared by the ray cast (raycast.cu) and the iso-surface extraction (marching_cubes.cu): block look-up,
-// voxel fetch by world position, and the trilinear sample both walk the volume with.  Reference (FL/ = FriedLiver/Source/):
-//   HashDataStruct::getHashEntryForSDFBlockPos, getVoxel(float3), worldToVirtualVoxelPos, virtualVoxelPosToLocalSDFBlockIndex   FL/DepthSensing/VoxelUtilHashSDF.h:226-234, 276-358, 407-485
+// voxel fetch by world position, and the trilinear sample both walk the volume with; the block geometry and the bucket walk are voxel_hash.cuh's.
+// Reference (FL/ = FriedLiver/Source/):
+//   HashDataStruct::getVoxel(float3)                                                                                         FL/DepthSensing/VoxelUtilHashSDF.h:407-418
 //   RayCastData::trilinearInterpolationSimpleFastFast                                                                        FL/DepthSensing/RayCastSDFUtil.h:100-121
 // Arithmetic contract: IEEE binary32, every operation individually rounded (TUs built -fmad=false, -prec-div=true), the reference's expression order.
 #pragma once
 #include "../../include/bf_tsdf.h"
 #include "bf_common.cuh"
+#include "voxel_hash.cuh"
 
 namespace bf {
 
-struct F3 { float x, y, z; };
-struct I3 { int x, y, z; };
 __device__ __forceinline__ F3 add3(F3 a, F3 b) { return F3{ a.x + b.x, a.y + b.y, a.z + b.z }; }
 __device__ __forceinline__ F3 sub3(F3 a, F3 b) { return F3{ a.x - b.x, a.y - b.y, a.z - b.z }; }
 __device__ __forceinline__ F3 scale3(float s, F3 a) { return F3{ s * a.x, s * a.y, s * a.z }; }
@@ -23,56 +23,28 @@ __device__ __forceinline__ F3 mul_dir(const float* M, F3 v) {        // xyz of f
     return F3{ M[0] * v.x + M[1] * v.y + M[2] * v.z + M[3] * 0.0f, M[4] * v.x + M[5] * v.y + M[6] * v.z + M[7] * 0.0f, M[8] * v.x + M[9] * v.y + M[10] * v.z + M[11] * 0.0f };
 }
 __device__ __forceinline__ int f2i_rz(float v) { return __float2int_rz(v); }                 // cvt.rzi.s32.f32: truncate, saturate, NaN -> 0
-__device__ __forceinline__ int isign(float v) { return (0.0f < v) - (v < 0.0f); }
 
 // ---- read-only hash access ----------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned hash_pos(unsigned numBuckets, I3 p) {                    // computeHashPos, VoxelUtilHashSDF.h:226-234
-    return (((unsigned)p.x * 73856093u) ^ ((unsigned)p.y * 19349669u) ^ ((unsigned)p.z * 83492791u)) % numBuckets;
-}
-__device__ __forceinline__ bool entry_is(const BFHashEntry* e, I3 p, int* ptr) {
-    const int4 q = __ldg(reinterpret_cast<const int4*>(e));                                   // pos.xyz, ptr: one 16-byte load (entries are 16-byte aligned)
-    if (q.x == p.x && q.y == p.y && q.z == p.z && q.w != BF_FREE_ENTRY) { *ptr = q.w; return true; }
-    return false;
-}
-// getHashEntryForSDFBlockPos, VoxelUtilHashSDF.h:440-485: the block's first-voxel index or BF_FREE_ENTRY
+// an entry read through the read-only path: pos.xyz and ptr in one 16-byte load (entries are 16-byte aligned), the offset only when the walk
+// follows it
+struct LdgEntry { int4 q; const BFHashEntry* e; };
+__device__ __forceinline__ bool entry_holds(const LdgEntry& e, I3 b) { return e.q.x == b.x && e.q.y == b.y && e.q.z == b.z && e.q.w != BF_FREE_ENTRY; }
+__device__ __forceinline__ unsigned entry_offset(const LdgEntry& e) { return __ldg(&e.e->offset); }
+// the block's first-voxel index or BF_FREE_ENTRY
 __device__ inline int find_block(const BFHashDataStruct& hd, const BFHashParams& hp, I3 b) {
-    const unsigned h = hash_pos(hp.m_hashNumBuckets, b), hpz = h * BF_HASH_BUCKET_SIZE, total = BF_HASH_BUCKET_SIZE * hp.m_hashNumBuckets;
-    int ptr;
-#pragma unroll
-    for (unsigned j = 0; j < BF_HASH_BUCKET_SIZE; ++j) if (entry_is(&hd.d_hash[hpz + j], b, &ptr)) return ptr;
-    const unsigned last = hpz + BF_HASH_BUCKET_SIZE - 1;
-    unsigned i = last;
-    for (unsigned it = 0; it < hp.m_hashMaxCollisionLinkedListSize; ++it) {
-        if (entry_is(&hd.d_hash[i], b, &ptr)) return ptr;
-        const unsigned off = __ldg(&hd.d_hash[i].offset);
-        if (off == 0) break;
-        i = (last + off) % total;
-    }
-    return BF_FREE_ENTRY;
+    const auto load = [&](unsigned i) { return LdgEntry{ __ldg(reinterpret_cast<const int4*>(&hd.d_hash[i])), &hd.d_hash[i] }; };
+    return walk_bucket(hp, b, hash_pos(hp.m_hashNumBuckets, b), load, [](const LdgEntry& e, unsigned) { return e.q.w; }, (int)BF_FREE_ENTRY);
 }
 struct BlockCache { I3 b; int ptr; bool valid; };
 struct VoxelW { float sdf, weight; unsigned color; };
-// worldToVirtualVoxelPos, :283-287
-__device__ __forceinline__ I3 world_to_voxel(const BFHashParams& hp, F3 pos) {
-    const float vs = hp.m_virtualVoxelSize;
-    const F3 p = { pos.x / vs, pos.y / vs, pos.z / vs };
-    return I3{ f2i_rz(p.x + (float)isign(p.x) * 0.5f), f2i_rz(p.y + (float)isign(p.y) * 0.5f), f2i_rz(p.z + (float)isign(p.z) * 0.5f) };
-}
 // the voxel at integer position v, with the thread's last block kept; a missing block reads as the empty voxel
 __device__ __forceinline__ VoxelW get_voxel_at(const BFHashDataStruct& hd, const BFHashParams& hp, I3 v, BlockCache& c) {
-    I3 t = v;                                                                                                                                 // virtualVoxelPosToSDFBlock, :290-299
-    if (t.x < 0) t.x -= BF_SDF_BLOCK_SIZE - 1;
-    if (t.y < 0) t.y -= BF_SDF_BLOCK_SIZE - 1;
-    if (t.z < 0) t.z -= BF_SDF_BLOCK_SIZE - 1;
-    const I3 b = { t.x / BF_SDF_BLOCK_SIZE, t.y / BF_SDF_BLOCK_SIZE, t.z / BF_SDF_BLOCK_SIZE };
+    const I3 b = voxel_to_block(v);
     if (!(c.valid && c.b.x == b.x && c.b.y == b.y && c.b.z == b.z)) { c.b = b; c.ptr = find_block(hd, hp, b); c.valid = true; }
     VoxelW r = { 0.0f, 0.0f, 0u };
     if (c.ptr == BF_FREE_ENTRY) return r;
-    I3 l = { v.x % BF_SDF_BLOCK_SIZE, v.y % BF_SDF_BLOCK_SIZE, v.z % BF_SDF_BLOCK_SIZE };                                                     // virtualVoxelPosToLocalSDFBlockIndex, :347-358
-    if (l.x < 0) l.x += BF_SDF_BLOCK_SIZE;
-    if (l.y < 0) l.y += BF_SDF_BLOCK_SIZE;
-    if (l.z < 0) l.z += BF_SDF_BLOCK_SIZE;
-    const unsigned* w = reinterpret_cast<const unsigned*>(hd.d_SDFBlocks + (size_t)c.ptr + (size_t)(l.z * BF_SDF_BLOCK_SIZE * BF_SDF_BLOCK_SIZE + l.y * BF_SDF_BLOCK_SIZE + l.x));
+    const int k = voxel_local_index(v);
+    const unsigned* w = reinterpret_cast<const unsigned*>(hd.d_SDFBlocks + (size_t)c.ptr + (size_t)k);
     r.sdf = __uint_as_float(__ldg(w)); r.weight = __uint_as_float(__ldg(w + 1)); r.color = __ldg(w + 2);
     return r;
 }

@@ -166,7 +166,7 @@ __device__ bool block_quad(const RcArgs& a, const BFHashEntry* e, F3& lo, F3& hi
     const I3 b = { q.x, q.y, q.z };
     if (!block_in_frustum(a.hp, a.cp, b)) return false;
     const float vs = a.hp.m_virtualVoxelSize;
-    const F3 wv = { (float)(b.x * BF_SDF_BLOCK_SIZE) * vs, (float)(b.y * BF_SDF_BLOCK_SIZE) * vs, (float)(b.z * BF_SDF_BLOCK_SIZE) * vs };
+    const F3 wv = block_to_world(a.hp, b);
     const F3 mn = { wv.x - vs / 2.0f, wv.y - vs / 2.0f, wv.z - vs / 2.0f };
     const F3 mx = { mn.x + (float)BF_SDF_BLOCK_SIZE * vs, mn.y + (float)BF_SDF_BLOCK_SIZE * vs, mn.z + (float)BF_SDF_BLOCK_SIZE * vs };
     lo = F3{ INFINITY, INFINITY, INFINITY }; hi = F3{ -INFINITY, -INFINITY, -INFINITY };

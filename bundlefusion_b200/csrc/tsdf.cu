@@ -28,6 +28,7 @@
 #include "tsdf_shared.cuh"
 #include "tsdf_keys.cuh"
 #include "tsdf_hash.cuh"
+#include "voxel_hash.cuh"
 #include "mat4.cuh"
 
 namespace bf {
@@ -94,12 +95,8 @@ static std::map<const void*, TsdfAux> g_aux;
 static int get_aux(const BFHashDataStruct* hd, const BFHashParams* hp, TsdfAux** out, bool create, bool adopt = true);
 
 // ------------------------------------------------------------------------------------------
-// device math shared by every kernel (bit-exact mirror of oracle/tsdf_oracle.c)
+// device math shared by every kernel (bit-exact mirror of oracle/tsdf_oracle.c); the block geometry is voxel_hash.cuh's
 // ------------------------------------------------------------------------------------------
-struct F3 { float x, y, z; };
-
-__device__ __forceinline__ int isign(float v) { return (0.0f < v) - (v < 0.0f); }
-
 // cuda_SimpleMatrixUtil.h:937-944 (affine, implicit w = 1), fused exactly as nvcc fuses the reference's expression
 // (oracle/tsdf_oracle.c header: the arithmetic contract); the TU is built -fmad=false so only these explicit FMAs fuse
 __device__ __forceinline__ F3 xform(const BFFloat4x4& M, F3 v) {
@@ -110,27 +107,6 @@ __device__ __forceinline__ F3 xform(const BFFloat4x4& M, F3 v) {
     return r;
 }
 __device__ __forceinline__ float truncation(const BFHashParams& hp, float z) { return __fmaf_rn(hp.m_truncScale, z, hp.m_truncation); }
-__device__ __forceinline__ I3 world_to_voxel(const BFHashParams& hp, F3 pos) {
-    F3 p = { pos.x / hp.m_virtualVoxelSize, pos.y / hp.m_virtualVoxelSize, pos.z / hp.m_virtualVoxelSize };
-    I3 r = { (int)(p.x + (float)isign(p.x) * 0.5f), (int)(p.y + (float)isign(p.y) * 0.5f), (int)(p.z + (float)isign(p.z) * 0.5f) };
-    return r;
-}
-__device__ __forceinline__ I3 voxel_to_block(I3 v) {
-    if (v.x < 0) v.x -= BF_SDF_BLOCK_SIZE - 1;
-    if (v.y < 0) v.y -= BF_SDF_BLOCK_SIZE - 1;
-    if (v.z < 0) v.z -= BF_SDF_BLOCK_SIZE - 1;
-    I3 r = { v.x / BF_SDF_BLOCK_SIZE, v.y / BF_SDF_BLOCK_SIZE, v.z / BF_SDF_BLOCK_SIZE };
-    return r;
-}
-__device__ __forceinline__ F3 voxel_to_world(const BFHashParams& hp, I3 v) {
-    F3 r = { (float)v.x * hp.m_virtualVoxelSize, (float)v.y * hp.m_virtualVoxelSize, (float)v.z * hp.m_virtualVoxelSize };
-    return r;
-}
-__device__ __forceinline__ F3 block_to_world(const BFHashParams& hp, I3 b) {
-    I3 v = { b.x * BF_SDF_BLOCK_SIZE, b.y * BF_SDF_BLOCK_SIZE, b.z * BF_SDF_BLOCK_SIZE };
-    return voxel_to_world(hp, v);
-}
-__device__ __forceinline__ I3 world_to_block(const BFHashParams& hp, F3 w) { return voxel_to_block(world_to_voxel(hp, w)); }
 
 __device__ __forceinline__ float proj_z(const BFDepthCameraParams& cp, float z) {
     return (z - cp.m_sensorDepthWorldMin) / (cp.m_sensorDepthWorldMax - cp.m_sensorDepthWorldMin);

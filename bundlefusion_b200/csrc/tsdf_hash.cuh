@@ -6,7 +6,7 @@
 
 #include "../../include/bf_tsdf.h"
 #include "tsdf_shared.cuh"
-#include "tsdf_keys.cuh"
+#include "tsdf_keys.cuh"          // and through it voxel_hash.cuh
 
 namespace bf {
 
@@ -15,9 +15,6 @@ namespace bf {
 // from L1 (possibly stale => at worst a spurious miss that is re-checked under the lock);
 // loads under a bucket lock use ld.global.cg (L2), stores are followed by __threadfence().
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool entry_matches(const BFHashEntry* e, I3 p) {
-    return e->pos[0] == p.x && e->pos[1] == p.y && e->pos[2] == p.z && e->ptr != BF_FREE_ENTRY;
-}
 __device__ __forceinline__ BFHashEntry load_entry_cg(const BFHashEntry* e) {
     BFHashEntry r;
     const int* s = reinterpret_cast<const int*>(e);
@@ -25,29 +22,13 @@ __device__ __forceinline__ BFHashEntry load_entry_cg(const BFHashEntry* e) {
     r.offset = (unsigned)__ldcg(s + 4);
     return r;
 }
-__device__ __forceinline__ bool entry_matches_v(const BFHashEntry& e, I3 p) {
-    return e.pos[0] == p.x && e.pos[1] == p.y && e.pos[2] == p.z && e.ptr != BF_FREE_ENTRY;
-}
 
-// VoxelUtilHashSDF.h:440-485 ; returns entry index or -1.  kCoherent: read through L2.
+// the entry index of block p in bucket h or its overflow list, or -1.  kCoherent: read through L2.
 template <bool kCoherent>
 __device__ int find_entry(const BFHashEntry* __restrict__ hash, const BFHashParams& hp, I3 p, unsigned h) {
-    const unsigned hpz = h * BF_HASH_BUCKET_SIZE;
-    const unsigned total = BF_HASH_BUCKET_SIZE * hp.m_hashNumBuckets;
-#pragma unroll
-    for (unsigned j = 0; j < BF_HASH_BUCKET_SIZE; ++j) {
-        if (kCoherent) { if (entry_matches_v(load_entry_cg(&hash[hpz + j]), p)) return (int)(hpz + j); }
-        else           { if (entry_matches(&hash[hpz + j], p)) return (int)(hpz + j); }
-    }
-    const unsigned last = hpz + BF_HASH_BUCKET_SIZE - 1;
-    unsigned i = last;
-    for (unsigned it = 0; it < hp.m_hashMaxCollisionLinkedListSize; ++it) {
-        BFHashEntry c = kCoherent ? load_entry_cg(&hash[i]) : hash[i];
-        if (entry_matches_v(c, p)) return (int)i;
-        if (c.offset == 0) break;
-        i = (last + c.offset) % total;
-    }
-    return -1;
+    const auto index = [](const BFHashEntry&, unsigned i) { return (int)i; };
+    if constexpr (kCoherent) return walk_bucket(hp, p, h, [&](unsigned i) { return load_entry_cg(&hash[i]); }, index, -1);
+    else return walk_bucket(hp, p, h, [&](unsigned i) -> const BFHashEntry& { return hash[i]; }, index, -1);
 }
 
 __device__ __forceinline__ bool try_lock(int* mutex) { return atomicCAS(mutex, BF_FREE_ENTRY, BF_LOCK_ENTRY) == BF_FREE_ENTRY; }
@@ -169,7 +150,7 @@ __device__ bool delete_entry(const BFHashDataStruct& hd, const BFHashParams& hp,
     for (unsigned j = 0; j < BF_HASH_BUCKET_SIZE && !ok; ++j) {
         const unsigned i = hpz + j;
         const BFHashEntry c = load_entry_cg(&hd.d_hash[i]);
-        if (entry_matches_v(c, p)) {
+        if (entry_holds(c, p)) {
             const unsigned slot = (unsigned)c.ptr / BF_SDF_BLOCK_VOXELS;
             const unsigned addr = atomicAdd(hd.d_heapCounter, 1u);            // appendHeap :541-546
             hd.d_heap[addr + 1] = slot;
@@ -192,7 +173,7 @@ __device__ bool delete_entry(const BFHashDataStruct& hd, const BFHashParams& hp,
         unsigned i = (last + c.offset) % total;
         for (unsigned it = 0; it < hp.m_hashMaxCollisionLinkedListSize; ++it) {
             c = load_entry_cg(&hd.d_hash[i]);
-            if (entry_matches_v(c, p)) {
+            if (entry_holds(c, p)) {
                 const unsigned slot = (unsigned)c.ptr / BF_SDF_BLOCK_VOXELS;
                 const unsigned addr = atomicAdd(hd.d_heapCounter, 1u);
                 hd.d_heap[addr + 1] = slot;

@@ -1,20 +1,13 @@
-// tsdf_keys.cuh -- SDF-block positions as packed 64-bit keys, the voxel hash's bucket function, and the device key set that
+// tsdf_keys.cuh -- SDF-block positions as packed 64-bit keys, bucket loads under the voxel hash's bucket function, and the device key set that
 // bfTsdfCountBlocks fills and bfTsdfBlockKeyLoad / bfTsdfBlockKeyMerge read (include/bf_tsdf.h).  Integer code only, so tsdf.cu
 // (built -fmad=false) includes it unchanged and the CPU suite compiles it against tests/cuda_emu.
 #pragma once
 #include <cuda_runtime.h>
 
 #include "../../include/bf_tsdf.h"
+#include "voxel_hash.cuh"
 
 namespace bf {
-
-struct I3 { int x, y, z; };
-
-// VoxelUtilHashSDF.h:226-234 (unsigned modulo, see oracle note)
-__device__ __forceinline__ unsigned hash_pos(unsigned numBuckets, I3 p) {
-    unsigned v = ((unsigned)p.x * 73856093u) ^ ((unsigned)p.y * 19349669u) ^ ((unsigned)p.z * 83492791u);
-    return v % numBuckets;
-}
 
 // key = bit 63 | three 21-bit fields biased by 2^20 (x, y, z from the top): a block with every coordinate in [-2^20, 2^20) packs, and
 // no key is 0, the key set's empty slot

@@ -24,6 +24,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from bundlefusion_b200 import _capi as capi  # noqa: E402
+from bundlefusion_b200 import fuse  # noqa: E402
 from bundlefusion_b200.frame_loop import FrameLoop, default_params  # noqa: E402
 from bundlefusion_b200.scene_rep import CUDASceneRepHashSDF  # noqa: E402
 from trajectory_fusion_timing import W, H, card, stream_bank  # noqa: E402
@@ -33,8 +34,8 @@ ENTRY, VOXEL_BLOCK = 32, 512 * 12
 
 
 def table_bytes(hp):
-    e = int(hp.m_hashNumBuckets) * 4
-    return 2 * ENTRY * e + 2 * 4 * e + 4 * int(hp.m_hashNumBuckets) + (4 + VOXEL_BLOCK) * int(hp.m_numSDFBlocks)
+    """the table's buckets (fuse.table_bytes), plus per heap block its heap word and voxel block"""
+    return fuse.table_bytes(int(hp.m_hashNumBuckets)) + (4 + VOXEL_BLOCK) * int(hp.m_numSDFBlocks)
 
 
 def hp_of(loop):

@@ -15,16 +15,23 @@ CSRC = os.path.join(ROOT, "bundlefusion_b200", "csrc")
 EMU = os.path.join(ROOT, "tests", "cuda_emu")
 
 
+def _splice(name: str, seen: set) -> str:
+    """csrc/`name` with the library's device headers it includes spliced in, recursively and each one once (bf_common.cuh, which the shim
+    replaces, is dropped)"""
+    if name in seen:
+        return ""
+    seen.add(name)
+    src = open(os.path.join(CSRC, name)).read().replace("#pragma once", "")
+    return re.sub(r'#include "(\w+\.cuh)"', lambda m: "" if m.group(1) == "bf_common.cuh" else _splice(m.group(1), seen), src)
+
+
 @functools.lru_cache(maxsize=None)
 def build_emulated(source: str, expected_launches: int, extra_pre: str = "", glue: str = "", sequential: bool = False) -> C.CDLL:
     """compile csrc/`source` (a .cu file, or a device header the `glue` launches from) for the CPU and load it.  `extra_pre` goes before the
     source, `glue` (the test's extern "C" wrappers) after it.  The source's <<<...>>> launches become EMU_LAUNCH, `expected_launches` of them.
     `sequential` runs each launch one CUDA thread after the other (BF_EMU_SEQUENTIAL, for sources that drop their warp collectives under it).
     One build per set of arguments and session."""
-    src = open(os.path.join(CSRC, source)).read()
-    # the library's own device headers are spliced in (they include bf_common.cuh, which the shim replaces)
-    src = re.sub(r'#include "(\w+\.cuh)"', lambda m: m.group(0) if m.group(1) == "bf_common.cuh" else open(os.path.join(CSRC, m.group(1))).read(), src)
-    src = src.replace('#include "bf_common.cuh"', "").replace("#pragma once", "")
+    src = _splice(source, set())
     src = re.sub(r"extern __shared__ float (\w+)\[\];", lambda m: "" if m.group(1) == "sm" else f"float* {m.group(1)} = sm;", src)      # dynamic shared memory: the shim's sm[]
     src = re.sub(r"extern __shared__ (unsigned|int) (\w+)\[\];", lambda m: f"{m.group(1)}* {m.group(2)} = reinterpret_cast<{m.group(1)}*>(sm);", src)
     src, n = re.subn(r"(\w+(?:<[\w\s,]+>)?)<<<\s*([^,]+),\s*([^,]+),\s*[^,]+,\s*[^>]+>>>\(", r"EMU_LAUNCH((\1), \2, \3, ", src)

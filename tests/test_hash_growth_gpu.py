@@ -3,7 +3,8 @@ table the model equals the source's keyed by block position, a garbage collectio
 list: a single integrate, a GC's stale list, a fused re-integration, a re-integration batch, an integrate batch and a bfTsdfRunOps replay -- and a
 further op list keeps the two equal; in fast and exact arithmetic and under a 2-rank shard setting.  The frame loop with growth on against a
 fixed table large enough never to drop: statuses, trajectory, op log and model bit for bit, after the steps and after finish(30), and the host
-synchronisation rule.  scan.py --grow-hash against a fixed large hash, and with a ceiling too small to hold the scan."""
+synchronisation rule.  A fixed table's loop hands the table's memory back when it is destroyed.  scan.py --grow-hash against a fixed large hash,
+and with a ceiling too small to hold the scan."""
 import ctypes as C
 import json
 
@@ -11,7 +12,7 @@ import numpy as np
 import pytest
 
 from bundlefusion_b200 import _capi as capi
-from bundlefusion_b200 import synth
+from bundlefusion_b200 import fuse, synth
 from bundlefusion_b200.frame_loop import FrameLoop
 from bundlefusion_b200.scene_rep import CUDASceneRepHashSDF, camera_params, default_hash_params
 from oracle import oracle as orc
@@ -248,6 +249,25 @@ def test_growth_adds_host_synchronisations_only_when_it_grows(cuda_device, loop_
     attempts = lambda g: g["growths"] + g["discarded"]
     assert grown["syncs"] - fixed["syncs"] == per * attempts(grown["growth"])
     assert grown["syncs_end"] - fixed["syncs_end"] == per * attempts(grown["growth_end"])
+
+
+def test_fixed_table_loop_hands_its_table_back(cuda_device):
+    """a fixed table comes from the same stream-ordered allocator as a growing one; destroying the loop returns it to the device"""
+    import torch
+    p = loop_params(N_LOOP)
+    assert p.hashMaxSDFBlocks == 0
+    table = fuse.table_bytes(p.hash.m_hashNumBuckets) + (4 + C.sizeof(capi.BFVoxel) * capi.BF_SDF_BLOCK_VOXELS) * p.hash.m_numSDFBlocks
+    FrameLoop(p, cuda_device).close()                           # the library's process-wide workspaces outlive the first loop
+    torch.cuda.synchronize(cuda_device)
+    before = torch.cuda.mem_get_info(cuda_device)[0]
+    loop = FrameLoop(p, cuda_device)
+    during = torch.cuda.mem_get_info(cuda_device)[0]
+    loop.close()
+    torch.cuda.synchronize(cuda_device)
+    after = torch.cuda.mem_get_info(cuda_device)[0]
+    print("free bytes: before %d, with the loop %d, after %d; table %d" % (before, during, after, table))
+    assert before - during >= table
+    assert abs(after - before) < table // 16, (before, after)
 
 
 def test_scan_grow_hash(cuda_device, recording, tmp_path, capsys):  # noqa: F811
